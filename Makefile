@@ -1,4 +1,4 @@
-# bnet build: host engine (g++) + sm_100a kernels (nvcc) -> libnccl-net.so
+# bnet build: host engine (g++) + sm_90a kernels (nvcc) -> libnccl-net.so
 #
 #   make            build the plugin / runtime library into bagua_net_b200/lib/
 #   make test       C++ unit + loopback tests (no GPU needed)
@@ -14,7 +14,7 @@
 CUDA_HOME ?= /usr/local/cuda
 NVCC      := $(CUDA_HOME)/bin/nvcc
 CXX       ?= g++
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 OUT       := bagua_net_b200/lib
 BUILD     := build
 
@@ -82,7 +82,7 @@ $(BUILD)/tests/nn_emu_test: csrc/tests/nn_emu_test.cc csrc/cuda/nn_body.cuh
 $(BUILD)/tests/exec_emu_test: csrc/tests/exec_emu_test.cc csrc/cuda/exec_body.cuh
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) $< -o $@
-# the tcgen05 linear kernel's index logic on an emulated TMA / MMA / TMEM
+# the wgmma linear kernel's index logic on an emulated TMA / MMA / accumulator
 $(BUILD)/tests/tc_emu_test: csrc/tests/tc_emu_test.cc csrc/cuda/tc_body.cuh include/bnet/bnet_tc.h
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) -Iinclude $< -o $@

@@ -1,12 +1,12 @@
-"""bagua_net_b200 — a Blackwell-native NCCL network transport + fused collectives.
+"""bagua_net_b200 — a Hopper-native NCCL network transport + fused collectives.
 
 Python face of the native library ``libnccl-net.so`` (C++ engine, multi-stream TCP
-transports, intra-host shared-memory/NVLink transport, sm_100a kernels):
+transports, intra-host shared-memory/NVLink transport, sm_90a kernels):
 
 * ``bagua_net_b200.utils``    — plugin loader, ctypes view of the ncclNet ABI tables,
   NIC discovery, telemetry readers, env helpers (what the reference exposes through
   environment variables only; reference: SURVEY.md §2.7).
-* ``bagua_net_b200.ops``      — hand-written sm_100a collectives/fused ops (NVLS
+* ``bagua_net_b200.ops``      — hand-written sm_90a collectives/fused ops (NVLS
   multimem all-reduce, P2P all-reduce, fused all-reduce+SGD, pack/cast).
 * ``bagua_net_b200.parallel`` — symmetric-memory communicator and the DDP engine
   that rides on those kernels (the reference's consumer is PyTorch/Bagua DDP,
@@ -31,7 +31,7 @@ def lib_path(name: str = LIB_NAME) -> str:
 
 
 def build(verbose: bool = False, jobs: int | None = None) -> str:
-    """Compile the native library in-tree (nvcc cross-compiles sm_100a without a GPU)."""
+    """Compile the native library in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     from ._build import build_native
 
     return build_native(verbose=verbose, jobs=jobs)

@@ -108,12 +108,12 @@ def run(out=sys.stdout) -> int:
     except Exception:
         ngpu = 0
     if ngpu == 0:
-        say(None, "CUDA", "no GPU visible: TCP and shared-memory transports only (the NVLink kernels need sm_100a)")
+        say(None, "CUDA", "no GPU visible: TCP and shared-memory transports only (the NVLink kernels need sm_90a)")
     else:
         import torch
 
         cap = torch.cuda.get_device_capability(0)
-        say(cap[0] >= 10, "GPU", f"{ngpu} x {torch.cuda.get_device_name(0)} (sm_{cap[0]}{cap[1]}); kernels are built for sm_100a")
+        say(tuple(cap) == (9, 0), "GPU", f"{ngpu} x {torch.cuda.get_device_name(0)} (sm_{cap[0]}{cap[1]}); kernels are built for sm_90a")
         if ngpu > 1:
             peer = all(torch.cuda.can_device_access_peer(0, j) for j in range(1, ngpu))
             say(peer, "peer access GPU0 -> others", "NVLink/PCIe P2P" if peer else "not available: the NVL direct path falls back to the staged ring")
@@ -132,11 +132,11 @@ def run(out=sys.stdout) -> int:
             from bagua_net_b200.ops import tc_conv
 
             v = tc_conv.prepare()
-            say(None, "tcgen05 kernels", f"linear / convolution self-check {'passed' if v['usable'] else 'not passed (cuBLAS / cuDNN are used)'}; "
+            say(None, "wgmma kernels", f"linear / convolution self-check {'passed' if v['usable'] else 'not passed (cuBLAS / cuDNN are used)'}; "
                 f"filter gradient {'trusted' if v['wgrad'] else 'not trusted'} on this GPU"
                 + (f" with {os.environ['BNET_TC_WGRAD_BN']}-column tiles" if v["wgrad"] and os.environ.get("BNET_TC_WGRAD_BN") else ""))
         except Exception as e:      # noqa: BLE001
-            say(None, "tcgen05 kernels", f"could not be checked: {e}")
+            say(None, "wgmma kernels", f"could not be checked: {e}")
         try:
             cu = ctypes.CDLL("libcuda.so.1")
             dev, val = ctypes.c_int(), ctypes.c_int()

@@ -16,7 +16,7 @@ class VGG(nn.Module):
     def __init__(self, cfg="vgg16", num_classes: int = 1000, batch_norm: bool = False, dropout: float = 0.5,
                  width_div: int = 1, fc_dim: int = 4096, image_size: int = 224, fused: bool = False):
         """fused=True builds the feature extractor from bagua_net_b200.ops.ConvBiasReLU blocks: bias, ReLU,
-        2x2 max-pool, their backward and the bias-gradient reduction run as one sm_100a pass each."""
+        2x2 max-pool, their backward and the bias-gradient reduction run as one sm_90a pass each."""
         super().__init__()
         layers, cin = [], 3
         spec = list(CFGS[cfg] if isinstance(cfg, str) else cfg)
@@ -52,7 +52,7 @@ class VGG(nn.Module):
         from ..ops import tc_linear
 
         if fused and tc_linear.enabled():
-            # opt-in (BNET_TC=1): Linear + bias + ReLU as one tcgen05 kernel; Identity keeps the Sequential indices —
+            # opt-in (BNET_TC=1): Linear + bias + ReLU as one wgmma kernel; Identity keeps the Sequential indices —
             # and so the state_dict keys — of the stock layout
             self.classifier = nn.Sequential(
                 tc_linear.TCLinear(cin * side * side, fc_dim, relu=True), nn.Identity(), nn.Dropout(dropout),

@@ -1,5 +1,5 @@
 """Fused conv-block layers (csrc/cuda/nn_kernels.cu): everything memory-bound that follows a
-convolution is folded into one sm_100a pass in forward and one in backward.
+convolution is folded into one sm_90a pass in forward and one in backward.
 
     ConvBiasReLU      y = relu(conv(x, w) + b)
     ConvBiasReLUPool  p = maxpool2x2(relu(conv(x, w) + b))      (y is never written to HBM)
@@ -29,19 +29,25 @@ def _L():
         _lib = load()
         vp, ll, i = C.c_void_p, C.c_longlong, C.c_int
         _lib.bnet_nn_bias_relu.argtypes = [vp, vp, ll, i, i, vp]
-        _lib.bnet_nn_relu_bwd_bias_grad.argtypes = [vp, vp, vp, vp, ll, i, i, vp]
+        _lib.bnet_nn_relu_bwd_bias_grad.argtypes = [vp, vp, vp, vp, vp, ll, i, i, vp]
         _lib.bnet_nn_bias_relu_pool_fwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp]
-        _lib.bnet_nn_pool_relu_bwd_bias_grad.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp]
+        _lib.bnet_nn_pool_relu_bwd_bias_grad.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, vp]
         f = C.c_float
-        _lib.bnet_nn_bn_stats.argtypes = [vp, vp, ll, i, i, vp]
+        _lib.bnet_nn_bn_stats.argtypes = [vp, vp, vp, ll, i, i, vp]
         _lib.bnet_nn_bn_apply.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, ll, i, f, f, i, i, vp]
-        _lib.bnet_nn_bn_bwd_reduce.argtypes = [vp, vp, vp, vp, vp, ll, i, f, i, i, vp]
+        _lib.bnet_nn_bn_bwd_reduce.argtypes = [vp, vp, vp, vp, vp, vp, ll, i, f, i, i, vp]
         _lib.bnet_nn_bn_bwd_apply.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ll, i, f, i, i, vp]
     return _lib
 
 
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _partials(ld: int, device) -> torch.Tensor:
+    """Workspace of a column reduction: one row of `ld` block partial sums per block, added up in block order by the library
+    (the same sums on every run); allocated on the current stream, so concurrent streams and graph captures get their own."""
+    return torch.empty((_L().bnet_nn_partial_rows(), ld), device=device, dtype=torch.float32)
 
 
 def _chk(rc, what):
@@ -65,8 +71,8 @@ def _conv(x, w, stride, padding):
 
 def _conv_backward(gz, x, w, stride, padding, need_x):
     """(gx, gw) of the convolution.  For 3x3 / stride 1 / pad 1 layers the autotuner (ops/tc_conv.py) decides per shape and
-    per gradient: the input gradient from the tcgen05 kernel (the filter is read as stored, MN-major, taps flipped), the
-    filter gradient from the tcgen05 kernel (64-pixel boxes of gz and x, split over the pixels) — or cuDNN for either."""
+    per gradient: the input gradient from the wgmma kernel (the filter is read as stored, MN-major, taps flipped), the
+    filter gradient from the wgmma kernel (64-pixel boxes of gz and x, split over the pixels) — or cuDNN for either."""
     def lib(want_x, want_w):
         return torch.ops.aten.convolution_backward(gz, x, w, None, stride, padding, [1, 1], False, [0, 0], 1, [want_x, want_w, False])
 
@@ -108,7 +114,7 @@ def _zero_bias(b: torch.Tensor) -> torch.Tensor:
 
 
 def _tc_fwd_chosen(x, w, b, stride, padding) -> bool:
-    """Did (or does, on first sight of this shape) the autotuner give this layer's forward convolution to the tcgen05 kernel?"""
+    """Did (or does, on first sight of this shape) the autotuner give this layer's forward convolution to the wgmma kernel?"""
     from . import tc_conv
 
     def lib():
@@ -127,7 +133,7 @@ def _is_3x3_s1p1(w, stride, padding) -> bool:
 
 
 def _conv_bias_relu(x, w, b, stride, padding):
-    """relu(conv(x, w) + b), NHWC: ONE tcgen05 kernel (bias + ReLU applied from TMEM) where the autotuner picked it for this
+    """relu(conv(x, w) + b), NHWC: ONE wgmma kernel (bias + ReLU applied in the epilogue) where the autotuner picked it for this
     shape, otherwise cuDNN's convolution followed by our in-place bias + ReLU pass."""
     def lib():
         z = _conv(x, w, stride, padding)
@@ -165,7 +171,8 @@ class _ConvBiasReLU(torch.autograd.Function):
         n, c, h, wd = y.shape
         gb = torch.zeros(c, device=y.device, dtype=torch.float32)
         gz = torch.empty_like(gy)
-        _chk(_L().bnet_nn_relu_bwd_bias_grad(gy.data_ptr(), y.data_ptr(), gz.data_ptr(), gb.data_ptr(), n * h * wd, c,
+        _chk(_L().bnet_nn_relu_bwd_bias_grad(gy.data_ptr(), y.data_ptr(), gz.data_ptr(), gb.data_ptr(),
+                                             _partials(c, y.device).data_ptr(), n * h * wd, c,
                                              _DT[y.dtype], _stream()), "relu_bwd_bias_grad")
         gx, gw = _conv_backward(gz, x, w, stride, padding, ctx.needs_input_grad[0])
         return gx, gw, gb.to(w.dtype), None, None
@@ -176,7 +183,7 @@ class _ConvBiasReLUPool(torch.autograd.Function):
     def forward(ctx, x, w, b, stride, padding):
         pool_bias = b
         if _is_3x3_s1p1(w, stride, padding) and x.dtype == torch.bfloat16 and _tc_fwd_chosen(x, w, b, stride, padding):
-            # the tcgen05 convolution has bias + ReLU in its epilogue: the pool pass sees relu(z + b) and adds nothing
+            # the wgmma convolution has bias + ReLU in its epilogue: the pool pass sees relu(z + b) and adds nothing
             from . import tc_conv
 
             z = tc_conv.conv3x3(x, w, b, relu=True)
@@ -204,7 +211,8 @@ class _ConvBiasReLUPool(torch.autograd.Function):
             gp = gp.contiguous(memory_format=torch.channels_last)
         gb = torch.zeros(c, device=gp.device, dtype=torch.float32)
         gz = torch.empty((n, c, h, wd), device=gp.device, dtype=gp.dtype, memory_format=torch.channels_last)
-        _chk(_L().bnet_nn_pool_relu_bwd_bias_grad(gp.data_ptr(), idx.data_ptr(), gz.data_ptr(), gb.data_ptr(), n, h, wd, c,
+        _chk(_L().bnet_nn_pool_relu_bwd_bias_grad(gp.data_ptr(), idx.data_ptr(), gz.data_ptr(), gb.data_ptr(),
+                                                  _partials(c, gp.device).data_ptr(), n, h, wd, c,
                                                   _DT[gp.dtype], _stream()), "pool_relu_bwd_bias_grad")
         gx, gw = _conv_backward(gz, x, w, stride, padding, ctx.needs_input_grad[0])
         return gx, gw, gb.to(w.dtype), None, None
@@ -221,7 +229,8 @@ class _ConvBNAct(torch.autograd.Function):
         n, c, h, wd = z.shape
         rows, dt, L = n * h * wd, _DT[z.dtype], _L()
         stats = torch.zeros(2 * c, device=z.device, dtype=torch.float32)
-        _chk(L.bnet_nn_bn_stats(z.data_ptr(), stats.data_ptr(), rows, c, dt, _stream()), "bn_stats")
+        _chk(L.bnet_nn_bn_stats(z.data_ptr(), stats.data_ptr(), _partials(2 * c, z.device).data_ptr(), rows, c, dt, _stream()),
+             "bn_stats")
         if res is not None and not _nhwc(res):
             res = res.contiguous(memory_format=torch.channels_last)
         y = torch.empty_like(z)
@@ -243,7 +252,8 @@ class _ConvBNAct(torch.autograd.Function):
         n, c, h, wd = z.shape
         rows, dt, L = n * h * wd, _DT[z.dtype], _L()
         gsum = torch.zeros(2 * c, device=z.device, dtype=torch.float32)
-        _chk(L.bnet_nn_bn_bwd_reduce(gy.data_ptr(), y.data_ptr(), z.data_ptr(), stats.data_ptr(), gsum.data_ptr(), rows, c, eps,
+        _chk(L.bnet_nn_bn_bwd_reduce(gy.data_ptr(), y.data_ptr(), z.data_ptr(), stats.data_ptr(), gsum.data_ptr(),
+                                     _partials(2 * c, z.device).data_ptr(), rows, c, eps,
                                      1 if relu else 0, dt, _stream()), "bn_bwd_reduce")
         gz = torch.empty_like(z)
         gres = torch.empty_like(z) if has_res else None

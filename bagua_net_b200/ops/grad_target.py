@@ -9,7 +9,7 @@ matching shape / dtype / layout, writes there and returns ``adopt(slice)`` — a
 autograd adopts without touching the data.  Everything else keeps working unchanged: the engine's hook copies a gradient that
 arrived in a tensor of its own into the slice (two passes instead of the add's three).
 
-The reference has no training engine (SURVEY.md section 2.5: data parallelism is its consumer); this belongs to the B200 side."""
+The reference has no training engine (SURVEY.md section 2.5: data parallelism is its consumer); this belongs to the GPU side."""
 from __future__ import annotations
 
 import weakref

@@ -1,19 +1,18 @@
-"""tcgen05 linear layer and the fused row-parallel (GEMM + all-reduce) linear (csrc/cuda/tc_gemm.cu).
+"""Tensor-core (wgmma) linear layer and the fused row-parallel (GEMM + all-reduce) linear (csrc/cuda/tc_gemm.cu).
 
     y = tc_linear.linear(x, w, bias, relu=True)                # bf16 [M,K] x [N,K]^T -> bf16 [M,N], fused bias + ReLU
     y = tc_linear.row_parallel_linear(x_k, w_k, comm)          # every rank holds a K-shard; fp32 sum lands on EVERY rank
     y = tc_linear.linear_reduce_scatter(x_k, w_k, comm)        # ... or only on the rank that owns each row block
     y = tc_linear.allgather_linear(x_rows, w, comm)            # x sharded by rows: peers' shards are TMA-loaded over NVLink
 
-The kernel stages operands with TMA (128-byte swizzle), multiplies with ``tcgen05.mma`` into TMEM and applies the
-epilogue straight out of TMEM; ``row_parallel_linear`` is the "compute step followed by a collective in ONE kernel"
+The kernel stages operands with TMA (128-byte swizzle), multiplies with ``wgmma.mma_async`` into register accumulators
+and applies the epilogue from there; ``row_parallel_linear`` is the "compute step followed by a collective in ONE kernel"
 form: the epilogue adds its fp32 tile into every rank's symmetric-heap output (``multimem.red`` through the NVSwitch
 multicast mapping, ``red.global`` per peer otherwise), so no separate all-reduce runs.
 
-The reference has no compute path (SURVEY.md §2.6) — this belongs to the B200 side of the framework.
+The reference has no compute path (SURVEY.md §2.6) — this belongs to the GPU side of the framework.
 
-STATUS: validated on B200 in round 2 (profiles/r2/tc_probe_1gpu.txt, profiles/r2/tc_linear_vs_cublas_1gpu.txt) and on by
-default (``BNET_TC=0`` disables); ``self_check()`` must pass on the GPU at hand before any caller trusts it
+On by default (``BNET_TC=0`` disables); ``self_check()`` must pass on the GPU at hand before any caller trusts it
 (``trusted()``), and every launch carries a device-side watchdog (``last_error()``)."""
 from __future__ import annotations
 
@@ -54,14 +53,12 @@ def _L():
         _lib.bnet_tc_last_error.restype = C.c_char_p
         _lib.bnet_tc_smem_desc.restype = C.c_uint64
         _lib.bnet_tc_smem_desc.argtypes = [C.c_uint32]
-        _lib.bnet_tc_instr_desc.restype = C.c_uint32
-        _lib.bnet_tc_instr_desc.argtypes = [i, i]
     return _lib
 
 
 def enabled() -> bool:
-    """Switch for callers (models, bench).  On by default since the kernel passed its probes on B200 hardware
-    (profiles/r2/tc_probe_1gpu.txt); BNET_TC=0 keeps every linear layer on cuBLAS."""
+    """Switch for callers (models, bench).  On by default (callers still wait for ``trusted()``); BNET_TC=0 keeps every
+    linear layer on cuBLAS."""
     return os.environ.get("BNET_TC", "1") == "1"
 
 
@@ -84,7 +81,7 @@ def _err_flag(dev: int) -> torch.Tensor:
 
 
 def last_error(device: int | None = None) -> int:
-    """Synchronises.  0 = every launch so far completed; 1/2/3 = the TMA producer / MMA issuer / epilogue gave up
+    """Synchronises.  0 = every launch so far completed; 1/2/3 = the TMA producer / the MMA warpgroups / a split-K slice waiting for its turn gave up
     waiting (the watchdog turned a stuck pipeline into this code).  Reading clears it."""
     dev = torch.cuda.current_device() if device is None else device
     f = _err_flag(dev)
@@ -137,7 +134,7 @@ def _splitk_scratch(device, M: int, N: int):
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, relu: bool = False,
            out: torch.Tensor | None = None, splits: int | None = None) -> torch.Tensor:
-    """``act(x @ w.T + bias)`` on the tcgen05 tensor cores; x [M,K], w [N,K] (torch ``Linear.weight``), bf16.
+    """``act(x @ w.T + bias)`` on the wgmma tensor cores; x [M,K], w [N,K] (torch ``Linear.weight``), bf16.
     ``splits``: K slices (None = automatic, see ``_auto_splits``; 1 = one pass with the epilogue fused in the kernel)."""
     global LAUNCHES
     _check_operands(x, w, bias)
@@ -208,7 +205,7 @@ def linear_wgrad(gy: torch.Tensor, x: torch.Tensor, out: torch.Tensor | None = N
 
 
 def _bwd_on_tc(gy, x, w) -> bool:
-    """The backward GEMMs run on the tcgen05 kernel too (BNET_TC_BWD=0 keeps them on cuBLAS) when the operands meet the
+    """The backward GEMMs run on the wgmma kernel too (BNET_TC_BWD=0 keeps them on cuBLAS) when the operands meet the
     TMA constraints: 16-byte row pitches, and more than 64 output features for dW."""
     if os.environ.get("BNET_TC_BWD", "1") != "1":
         return False
@@ -219,7 +216,7 @@ def _bwd_on_tc(gy, x, w) -> bool:
 
 def weight_grad(gy: torch.Tensor, x: torch.Tensor, w: torch.Tensor, tc: bool) -> torch.Tensor:
     """dW = gy.T @ x of a linear layer.  When a training engine registered a gradient slice for `w` (ops/grad_target.py) the
-    GEMM writes straight into it — the tcgen05 kernel through its output pointer, cuBLAS through ``out=`` — and the slice is
+    GEMM writes straight into it — the wgmma kernel through its output pointer, cuBLAS through ``out=`` — and the slice is
     handed to autograd for adoption: no tensor of its own, no accumulate pass over the (for VGG16's fc1: 205 MB) gradient."""
     from . import grad_target
 
@@ -236,7 +233,7 @@ def weight_grad(gy: torch.Tensor, x: torch.Tensor, w: torch.Tensor, tc: bool) ->
 
 
 class _LinearAct(torch.autograd.Function):
-    """Forward on the tcgen05 kernel (bias and ReLU in its epilogue); dX and dW on the same kernel with MN-major
+    """Forward on the wgmma kernel (bias and ReLU in its epilogue); dX and dW on the same kernel with MN-major
     operands (no transposed copies), or on cuBLAS when the shapes do not meet the TMA constraints."""
 
     @staticmethod
@@ -350,7 +347,7 @@ def trusted() -> bool:
 
 class TCLinear(torch.nn.Linear):
     """``nn.Linear`` (same parameters, same state_dict keys) with an optional fused ReLU whose forward runs on the
-    tcgen05 kernel when ``BNET_TC=1`` and the self-check passed on this GPU; cuBLAS + eager ReLU otherwise."""
+    wgmma kernel when ``BNET_TC=1`` and the self-check passed on this GPU; cuBLAS + eager ReLU otherwise."""
 
     def __init__(self, in_features, out_features, bias=True, relu=False, **kw):
         super().__init__(in_features, out_features, bias=bias, **kw)
@@ -364,7 +361,7 @@ class TCLinear(torch.nn.Linear):
         return torch.relu(y) if self.relu else y
 
     def extra_repr(self):
-        return super().extra_repr() + f", relu={self.relu}, tcgen05={'on' if enabled() else 'off'}"
+        return super().extra_repr() + f", relu={self.relu}, wgmma={'on' if enabled() else 'off'}"
 
 
 def row_parallel_linear(x: torch.Tensor, w: torch.Tensor, comm, bias: torch.Tensor | None = None,

@@ -2,7 +2,7 @@
 
 One process per GPU.  Every rank allocates the same-sized heap with the CUDA VMM API,
 the allocations are exchanged as POSIX fds and mapped into every peer (NVLink P2P), and —
-when the fabric exposes it — bound to one multicast object so that the sm_100a kernels
+when the fabric exposes it — bound to one multicast object so that the sm_90a kernels
 can reduce inside the NVSwitch (multimem.ld_reduce) and broadcast through it
 (multimem.st).  ``torch.distributed`` is only the control plane that carries the
 128-byte handshake blobs (csrc/cuda/coll.cu, include/bnet/bnet_coll.h).
@@ -86,7 +86,7 @@ class SymmComm:
 
     def __init__(self, heap_bytes: int, device: int | None = None, group=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("bagua_net_b200 collectives need a CUDA device (sm_100a); none is visible")
+            raise RuntimeError("bagua_net_b200 collectives need a CUDA device (sm_90a); none is visible")
         self.lib = load()
         _declare(self.lib)
         self.group = group

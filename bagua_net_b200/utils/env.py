@@ -14,8 +14,7 @@ from .. import LIB_DIR
 
 
 # NCCL drives a net plugin through a proxy pipeline of NCCL_BUFFSIZE/8-byte slices per channel; with the default
-# 4 MiB buffers and 2-4 channels that pipeline, not the link, bounds the throughput (measured on 2 x B200:
-# 82 GB/s default -> 211 GB/s with these, profiles/README.md section 4)
+# 4 MiB buffers and 2-4 channels that pipeline, not the link, bounds the throughput
 TUNED = {"NCCL_BUFFSIZE": str(32 << 20), "NCCL_MIN_NCHANNELS": "16", "NCCL_PROTO": "Simple"}
 
 
@@ -42,8 +41,8 @@ def nccl_plugin_env(plugin: str = "bnet", force_net: bool = False, gdr: bool = T
     if eager_modules and "CUDA_MODULE_LOADING" not in os.environ:
         # CUDA loads kernels lazily, and the first launch of a kernel waits for the device to drain.  If the APPLICATION
         # launches a kernel for the first time while a collective is in flight, that wait never ends: the NCCL kernel is
-        # waiting for this transport's copy kernel, whose launch sits behind the loader (measured on 2 x B200 with torch
-        # DDP: proxy thread 26 s inside cudaLaunchKernelEx, profiles/README.md).  Stock NCCL never launches from its
+        # waiting for this transport's copy kernel, whose launch sits behind the loader (seen under torch DDP: the
+        # proxy thread stuck inside cudaLaunchKernelEx).  Stock NCCL never launches from its
         # proxy, so it is immune; a transport that moves data with kernels needs every module loaded up front.
         # The price is start-up time (torch + cuDNN + cuBLAS hold gigabytes of kernels: 100 s per process measured with
         # 2 ranks, 260 s with 4).  eager_modules=False leaves loading lazy: then the APPLICATION has to launch each of

@@ -3,7 +3,7 @@
 
 The reference's headline number is VGG16 synthetic training img/s with its plugin under NCCL
 (reference README.md:52-84; BASELINE.md: 4046.6 img/s on 32 x V100 / 100 GbE).  This script
-measures the same metric on N B200s of one box:
+measures the same metric on N H100s of one box:
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -70,7 +70,7 @@ def headline_line(reason: str | None = None) -> str:
            "config": {"model": a.model, "global_batch": h["world"] * a.batch, "per_gpu_batch": a.batch, "seq_len": None,
                       "image": [3, a.image, a.image], "parallelism": f"dp{h['world']}", "comm": a.comm, "path": h["path"],
                       "fused_conv_blocks": h["fused"], "cuda_graph": h["graph_used"], "params": h["n_params"],
-                      "l2": "no explicit flush: per-step working set (553 MB params+grads, activations) exceeds the 126 MB L2",
+                      "l2": "no explicit flush: per-step working set (553 MB params+grads, activations) exceeds the 50 MB L2",
                       **({"safe_level": int(os.environ["BNET_BENCH_SAFE_LEVEL"])} if os.environ.get("BNET_BENCH_SAFE_LEVEL") else {})},
            "clocks": h["clocks"], "gpu_launches": h["nlaunch"], "wall_ms_per_step": round(h["wall_ms"], 3)}
     if h.get("checksum"):
@@ -152,7 +152,7 @@ def reference_arm(args):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -376,11 +376,32 @@ def run_child_arm(comm_name: str, args, rank: int, world: int, port_offset: int,
 
 
 # What a failed run is repeated with (1 GPU only; a fresh process, because a faulting kernel poisons the CUDA context):
-# level 1 switches off what had not run on hardware when this round's GPU budget ended (adopted gradients, the tcgen05 filter
-# gradient), level 2 every tcgen05 kernel and the CUDA graph.  The JSON line says which level produced the number
+# level 1 switches off what had not run on hardware when this round's GPU budget ended (adopted gradients, the wgmma filter
+# gradient), level 2 every wgmma kernel and the CUDA graph.  The JSON line says which level produced the number
 # (config.safe_level); the run itself is the full benchmark either way — same model, same step, same optimizer.
 SAFE_LEVELS = ({"BNET_DIRECT_GRADS": "0", "BNET_TC_WGRAD": "0"},
                {"BNET_DIRECT_GRADS": "0", "BNET_TC_WGRAD": "0", "BNET_TC": "0", "BNET_TC_CONV": "0", "BNET_BENCH_NO_GRAPH": "1"})
+
+
+DUMP_PARAM_SAMPLE = 1 << 22       # float32 elements of the parameter sample: 16 MiB
+
+
+def dump_outputs(out_dir: str, loss, params) -> None:
+    """What a caller of the timed training step receives after its last step: the loss it returned and the parameters it
+    updated (a fixed, seeded sample of them when there are more than DUMP_PARAM_SAMPLE), as float32 .npy files."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    loss = loss if torch.is_tensor(loss) else torch.tensor(loss)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    flat = params.detach().reshape(-1)
+    if flat.numel() > DUMP_PARAM_SAMPLE:
+        gen = torch.Generator().manual_seed(0)
+        idx = torch.randint(0, flat.numel(), (DUMP_PARAM_SAMPLE,), generator=gen).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat.float().cpu().numpy())
+    note(f"outputs of the last timed step written to {out_dir}")
 
 
 def main() -> int:
@@ -430,10 +451,15 @@ def _main() -> int:
                     help="no ResNet-50 arm starts once the run is this many seconds old")
     ap.add_argument("--no-prefetch", action="store_true", help="e2e: per-step API instead of the prefetching loop")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel of the step individually (no CUDA graph)")
-    ap.add_argument("--no-fused", action="store_true", help="eager bias/ReLU/pool instead of the fused sm_100a conv blocks")
+    ap.add_argument("--no-fused", action="store_true", help="eager bias/ReLU/pool instead of the fused sm_90a conv blocks")
     ap.add_argument("--force-fused", action="store_true", help="resnet: skip the fused-vs-eager timing and use the fused blocks")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the last timed step computed (loss, a fixed sample of the updated "
+                         "parameters) as DIR/<name>.npy")
     ap.add_argument("--child-json", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return reference_arm(args)
     if args.warmup < 3:
@@ -459,14 +485,17 @@ def _main() -> int:
     if world != args.gpus and rank == 0:
         print(f"[bench] note: --gpus {args.gpus} but WORLD_SIZE={world}; using WORLD_SIZE", file=sys.stderr)
     if not torch.cuda.is_available():
-        print(json.dumps({"error": "no CUDA device visible; bench.py needs a B200"}), flush=True)
+        print(json.dumps({"error": "no CUDA device visible; bench.py needs an H100"}), flush=True)
         return 2
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     note(f"start: comm={args.comm} model={args.model} world={world}")
     init_process_group_from_env("nccl")
     note("process group up")
-    torch.backends.cudnn.benchmark = True
+    # cuDNN's algorithms by its heuristics and among the deterministic ones only: with the same arguments every run computes
+    # the same numbers (benchmark mode would pick by timing, run by run)
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.backends.cudnn.allow_tf32 = True
     torch.manual_seed(1234)
@@ -499,7 +528,7 @@ def _main() -> int:
             if rank == 0:
                 print(f"[bench] WARNING: {fused_note}", file=sys.stderr)
     if fused:
-        # settle the tcgen05 kernels' once-per-process verdicts (the filter gradient's runs in a child process the first
+        # settle the wgmma kernels' once-per-process verdicts (the filter gradient's runs in a child process the first
         # time on a machine) while no collective is in flight, then line the ranks up again
         from bagua_net_b200.ops import tc_conv
 
@@ -512,9 +541,9 @@ def _main() -> int:
                       [(64, 64, s_ // 4), (128, 128, s_ // 8), (256, 256, s_ // 16), (512, 512, s_ // 32)])
             os.environ["BNET_TC_WGRAD_CHECK_SHAPES"] = ";".join(f"{args.batch},{ci},{co},{hw}" for ci, co, hw in layers if hw > 0)
         try:
-            note(f"tcgen05 kernels: {tc_conv.prepare()}")
+            note(f"wgmma kernels: {tc_conv.prepare()}")
         except Exception as ex:   # noqa: BLE001 - an unsettled verdict only means cuDNN / cuBLAS are used
-            note(f"tcgen05 kernels: verdicts could not be settled ({ex!r})")
+            note(f"wgmma kernels: verdicts could not be settled ({ex!r})")
         if world > 1:
             dist.barrier()
     if fused and args.model.startswith("resnet") and not args.force_fused:
@@ -761,9 +790,12 @@ def _main() -> int:
     if sampler:
         sampler.start()
     l0 = launches()
-    ms_total, wall_total = timed(lambda: step_dev(x_dev, y_dev), args.steps)
+    last = {}
+    ms_total, wall_total = timed(lambda: last.__setitem__("loss", step_dev(x_dev, y_dev)), args.steps)
     nlaunch = launches() - l0
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], param_vector())
     ms_step = ms_total / args.steps
     img_s = world * B / (ms_step / 1e3)
 
@@ -825,7 +857,7 @@ def _main() -> int:
                         # with this many ranks is measured here, on this box: same kernel, same check (max over ranks), the
                         # fastest count is reported together with the default's time.
                         tried = {"default": round(ms / iters * 1e3, 1)}
-                        for nb in (48, 64, 96, 148):
+                        for nb in (48, 64, 96, 132):
                             for _ in range(3):
                                 comm.all_reduce(t, "sum", nblocks=nb)
                             ms_nb, _ = timed(lambda: comm.all_reduce(t, "sum", nblocks=nb), iters)
@@ -843,7 +875,8 @@ def _main() -> int:
                 # bytes per direction per GPU: in-switch path S(1+1/n), direct two-shot S(n-1)/n
                 per_dir = (1 + 1 / world) if path == "nvls" else (world - 1) / world
                 extra["allreduce_algo"] = path
-                extra["allreduce_roofline_frac_of_770GBs"] = {k: round(v / (2 * (world - 1) / world) * per_dir / 770.0, 3)
+                # against the nominal NVLink 4 bandwidth of an H100 SXM, 450 GB/s per direction (data sheet, not a measured peak)
+                extra["allreduce_roofline_frac_of_450GBs"] = {k: round(v / (2 * (world - 1) / world) * per_dir / 450.0, 3)
                                                               for k, v in bw.items() if int(k) >= (1 << 20)}
             except Exception as ex:   # the headline number must survive a failing side measurement
                 extra["allreduce_error"] = str(ex)[:200]
@@ -946,7 +979,7 @@ def _main() -> int:
         #      (host pointers only: NCCL stages through host memory; multi-stream TCP, here over the loopback interface; no NVLink or
         #      shared-memory transport).  The reference itself cannot be built here (--impl reference says why); this is its product
         #      re-implemented, same model, same step, so the ratio to the headline is the same-box speed-up over "what the
-        #      reference gives on an 8 x B200 node".
+        #      reference gives on an 8 x H100 node".
         if (args.comm == "bnet" and world > 1 and not args.no_arms and not args.no_resnet and not os.environ.get("BNET_BENCH_CHILD")):
             sync_all()
             go = torch.tensor([1 if time.time() - _T0 < args.resnet_deadline else 0], device=dev, dtype=torch.int32)
@@ -1031,7 +1064,7 @@ def _main() -> int:
                        "optimizer": opt_desc, "params": n_params, "bucket_mb": args.bucket_mb,
                        **({"safe_level": int(os.environ["BNET_BENCH_SAFE_LEVEL"]),
                            "safe_reason": os.environ.get("BNET_BENCH_SAFE_REASON")} if os.environ.get("BNET_BENCH_SAFE_LEVEL") else {}),
-                       "l2": "no explicit flush: per-step working set (553 MB params+grads, activations) exceeds the 126 MB L2",
+                       "l2": "no explicit flush: per-step working set (553 MB params+grads, activations) exceeds the 50 MB L2",
                        "baseline": "4046.6 img/s on 32xV100/100GbE (reference README.md:68)"},
             "clocks": clocks, "gpu_launches": nlaunch, "wall_ms_per_step": round(wall_total / args.steps, 3),
             "param_checksum": checksum,
@@ -1048,7 +1081,7 @@ def _main() -> int:
             except Exception:   # noqa: BLE001 - reporting only
                 pass
         try:
-            # what the per-shape autotuner measured on THIS GPU (tcgen05 kernel vs cuDNN, us) and which one the step runs
+            # what the per-shape autotuner measured on THIS GPU (wgmma kernel vs cuDNN, us) and which one the step runs
             from bagua_net_b200.ops import tc_conv
 
             if tc_conv.TIMINGS or tc_conv._choice:

@@ -7,8 +7,8 @@ events, max over ranks, reported against the NVLink roofline.
       bench/allreduce_sweep.py [--min-bytes 1K --max-bytes 1G --dtype bf16 --blocks 0 --json out.json]
 
 Roofline: an in-switch (NVLS) all-reduce of S bytes moves S(1+1/n) bytes in and out of every GPU;
-a P2P two-shot moves 2S(n-1)/n.  Link bandwidth = the measured 770 GB/s per direction per GPU
-(B200_PROFILING.md; 900 GB/s nominal).
+a P2P two-shot moves 2S(n-1)/n.  Link bandwidth = 450 GB/s per direction per GPU, the nominal NVLink 4 figure of an
+H100 SXM (data sheet; not a measured peak).
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ import torch.distributed as dist
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from bagua_net_b200.parallel import SymmComm, init_process_group_from_env  # noqa: E402
 
-LINK_GBS = 770.0
+LINK_GBS = 450.0          # nominal, H100 SXM NVLink 4 per direction
 
 
 def parse_size(s: str) -> int:

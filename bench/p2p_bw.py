@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """NVLink peer bandwidth of the transport executor (K1) and of the fused ops (K4/K5):
-rank 0 pushes from its own heap into rank 1's heap through the same sm_100a cluster kernels
+rank 0 pushes from its own heap into rank 1's heap through the same sm_90a cluster kernels
 that serve the plugin's isend.  Launch with torchrun on >= 2 GPUs.
 
   python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 bench/p2p_bw.py

@@ -23,7 +23,7 @@ static int copy_out(const std::string& s, char* out, int cap) {
   return (int)s.size();
 }
 
-BNET_API const char* bnet_version() { return "bnet 0.2 (sm_100a)"; }
+BNET_API const char* bnet_version() { return "bnet 0.2 (sm_90a)"; }
 
 BNET_API unsigned long long bnet_chunk_size(unsigned long long total, unsigned long long min_chunk,
                                             unsigned long long nchunks) {

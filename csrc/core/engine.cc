@@ -229,7 +229,7 @@ int Engine::init() {
   // Device model (SURVEY section 5.8).  The reference has one NCCL device per NIC (reference nthread_…:241-257).
   // On an NVSwitch box the "NIC" of a GPU is its own NVLink port, so when the device path is usable every visible
   // GPU gets a virtual device of its own (guid per GPU, NVLink speed).  It carries NO pciPath: a <nic> under the GPU's
-  // own <pci> node crashes NCCL's topology code (profiles/README.md R2.2), so GPUDirect is enabled by the
+  // own <pci> node crashes NCCL's topology code, so GPUDirect is enabled by the
   // NCCL_NET_GDR_LEVEL=SYS default the plugin's init supplies instead of by PCI distance.  Every virtual device keeps a
   // TCP side on a real interface (cross-host peers, fallbacks); the plain NIC devices follow after them.
   std::vector<NetIf> nics = find_interfaces();
@@ -260,7 +260,7 @@ int Engine::init() {
       p.pci_path = own_path ? path : std::string();
       p.guid = fnv1a(busid.data(), busid.size()) ^ (uint64_t)g;
       p.ptr_support = NCCL_PTR_HOST | NCCL_PTR_CUDA;
-      p.speed_mbps = speed_override > 0 ? (int)speed_override : 7200000;   // 900 GB/s per direction (NVLink 5)
+      p.speed_mbps = speed_override > 0 ? (int)speed_override : 3600000;   // 450 GB/s per direction (H100 NVLink 4)
       p.port = 0;
       p.latency_us = 0;
       p.max_comms = 65536;
@@ -277,7 +277,7 @@ int Engine::init() {
     p.guid = i;  // reference: guid = device index (nthread_…:250)
     p.ptr_support = NCCL_PTR_HOST | (cuda_ok_ ? NCCL_PTR_CUDA : 0);
     p.speed_mbps = nics[i].speed_mbps;
-    // With the NVLink path available the "wire" is NVLink 5, not the NIC.
+    // With the NVLink path available the "wire" is NVLink, not the NIC.
     if (cfg.nvl && cuda_ok_ && !gpu_devs) p.speed_mbps = 1600000;
     if (speed_override > 0) p.speed_mbps = (int)speed_override;
     p.port = 0;

@@ -1,4 +1,4 @@
-// bnet collectives: symmetric-heap communicator + fused sm_100a kernels (K4/K5/K6).
+// bnet collectives: symmetric-heap communicator + fused sm_90a kernels (K4/K5/K6).
 //
 //   * NVLS all-reduce: multimem.ld_reduce (reduction inside the NVSwitch) followed by
 //     multimem.st (switch broadcast) on a cuMulticast mapping of the symmetric heap —
@@ -662,14 +662,14 @@ int launch(K kernel, int nblocks, int threads, cudaStream_t st, Args... args) {
   return 1;
 }
 
-// CTA counts measured on 2 x B200 (profiles/allreduce_sweep_2gpu.txt): the in-switch (multimem) kernels
-// peak at ~32 CTAs and lose bandwidth with more; the peer load/store kernels keep gaining up to one CTA
-// per SM; a single GPU has no fabric to wait for but all of HBM to feed: 2 CTAs per SM.
+// Default CTA counts (BNET_COLL_BLOCKS_* override them): the in-switch (multimem) kernels only issue requests
+// to the switch and get 32 CTAs; the peer load/store kernels get one CTA per SM of an H100 (132); a single GPU has
+// no fabric to wait for but all of HBM to feed: 2 CTAs per SM.
 enum BlockClass { BLK_NVLS = 0, BLK_P2P = 1, BLK_FUSED_NVLS = 2, BLK_SINGLE = 3 };
 int pick_blocks(const BnetColl* c, size_t vec_per_rank, int requested, BlockClass cls) {
   if (requested > 0) return requested > BNET_COLL_MAX_BLOCKS ? BNET_COLL_MAX_BLOCKS : requested;
-  static const int caps[4] = {(int)env_int("COLL_BLOCKS_NVLS", 32), (int)env_int("COLL_BLOCKS_P2P", 148),
-                              (int)env_int("COLL_BLOCKS_FUSED_NVLS", 64), (int)env_int("COLL_BLOCKS_SINGLE", 296)};
+  static const int caps[4] = {(int)env_int("COLL_BLOCKS_NVLS", 32), (int)env_int("COLL_BLOCKS_P2P", 132),
+                              (int)env_int("COLL_BLOCKS_FUSED_NVLS", 64), (int)env_int("COLL_BLOCKS_SINGLE", 264)};
   int cap = c->world == 1 ? caps[BLK_SINGLE] : caps[cls];
   if (cap > BNET_COLL_MAX_BLOCKS) cap = BNET_COLL_MAX_BLOCKS;
   if (cap < 1) cap = 1;

@@ -1,5 +1,5 @@
 // Narrow interface between the host engine (plain C++) and the CUDA side
-// (runtime + driver API + sm_100a kernels).  Everything degrades to "not
+// (runtime + driver API + sm_90a kernels).  Everything degrades to "not
 // available" on a box without a GPU/driver so the TCP + shared-memory paths and
 // all CPU tests keep working.
 #pragma once

@@ -2,11 +2,11 @@
 // of a job — copy (K1), move + accumulate (K4), move + cast (K5), fp8 gradient compression.
 //
 // Written as functions of (tid, nthreads) with the PTX accesses behind __CUDA_ARCH__ switches, so that the
-// SAME code is inlined into the sm_100a kernels by nvcc and compiled by g++ for csrc/tests/exec_emu_test.cc,
+// SAME code is inlined into the sm_90a kernels by nvcc and compiled by g++ for csrc/tests/exec_emu_test.cc,
 // which walks an emulated CTA over every op, size and alignment on the CPU (`make test`, no GPU needed).
 //
 // Memory-level parallelism: every vector loop is `batched<U>` — U 16-byte loads are issued before the first
-// dependent instruction (the reductions/stores that follow are fire-and-forget), see profiles/README.md.
+// dependent instruction (the reductions/stores that follow are fire-and-forget).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
@@ -270,8 +270,7 @@ BNET_XD_FN void process_range(uint32_t op, const char* src, char* dst, size_t n,
       size_t nv = ne >> 3;   // 8 bf16 in, 2 x float4 out
       // Lane-interleaved inside blocks of 32 vectors (256 elements): vector l of a block takes elements [4l, 4l+4) and
       // [128+4l, 128+4l+4).  Each of a warp's two output instructions then covers 512 CONTIGUOUS bytes (whole sectors,
-      // full NVLink packets) instead of 16 bytes out of every 32 — the plain mapping ran at half the red.add rate
-      // (ncu + timing: profiles/README.md R2.6).
+      // full NVLink packets) instead of 16 bytes out of every 32 as the plain mapping did.
       const size_t nblk = nv & ~(size_t)31;
       xb::batched<8, int4>(nblk, tid, nthreads,
                            [&](size_t i) {

@@ -5,7 +5,7 @@
 // and (b) compiled by g++ and driven over an emulated grid by csrc/tests/nn_emu_test.cc — the CPU check of
 // the indexing, masking and index-coding logic that `make test` runs without a GPU.
 //
-// Memory-level parallelism rule used below (measured: profiles/README.md section 5): issue ALL the 16-byte
+// Memory-level parallelism rule used below: issue ALL the 16-byte
 // loads of an unrolled batch as raw vectors first, convert/compute afterwards.  Converting right after each
 // load makes the next load wait behind the first one's latency and leaves the kernel at ~30% of HBM bandwidth.
 #pragma once

@@ -1,9 +1,8 @@
-// Fused memory-bound layers of the benchmark models (channels_last / NHWC), sm_100a.
+// Fused memory-bound layers of the benchmark models (channels_last / NHWC), sm_90a.
 //
-// profiles/step_profile_torch.txt: in an eager VGG16 bf16 step on B200 the tensor-core convolutions
-// are ~30% of the time; bias-add, ReLU, max-pool, their backward passes and the bias-gradient
-// reductions — all HBM-bound, one full pass over the activations each — are > 50%.  These kernels
-// fuse every such chain behind a convolution into ONE pass:
+// In an eager VGG16 bf16 step, bias-add, ReLU, max-pool, their backward passes and the bias-gradient
+// reductions are all HBM-bound, one full pass over the activations each.  These kernels fuse every such
+// chain behind a convolution into ONE pass:
 //   forward : z = conv(x,w)  ->  y = relu(z + b)                      (in place, 1 read + 1 write)
 //             z = conv(x,w)  ->  p = maxpool2x2(relu(z + b)), idx      (y is never materialised)
 //   backward: gz = gy * (y > 0)  and  gb = sum(gz)                     (1 pass instead of 2.3)
@@ -29,9 +28,11 @@ __global__ void __launch_bounds__(256) bias_relu_kernel(T* __restrict__ z, const
   bias_relu_thread<T>(z, bias, nvec, cvec, (size_t)blockIdx.x * blockDim.x + threadIdx.x, (size_t)gridDim.x * blockDim.x);
 }
 
-// block-wide reduction of per-thread channel-group sums, then one atomic per channel per block
+// block-wide reduction of per-thread channel-group sums; the block stores its partial sums at row blockIdx.x (pitch `ld`
+// floats) of `part`, and sum_rows_kernel adds the rows up in block order.  Atomics would add them in whatever order the
+// blocks finish, and the gradient would then differ in its last bits from run to run.
 template <int V>
-__device__ __forceinline__ void reduce_bias_grad(float* acc, float* __restrict__ gb, int cvec, float* smem) {
+__device__ __forceinline__ void reduce_bias_grad(float* acc, float* __restrict__ part, int ld, int cvec, float* smem) {
   const int rows = blockDim.x / cvec;           // threads that share a channel group
   const int grp = threadIdx.x % cvec, trow = threadIdx.x / cvec;
 #pragma unroll
@@ -44,13 +45,27 @@ __device__ __forceinline__ void reduce_bias_grad(float* acc, float* __restrict__
     for (int r = 0; r < rows; r++)
 #pragma unroll
       for (int k = 0; k < V; k++) s[k] += smem[(r * cvec + grp) * V + k];
-    // 16-byte reductions: a quarter of the atomic operations of scalar adds.  Same-cache-line atomics serialise in the L2
-    // slice that owns the line (measured: the 512-channel layers spent ~60 of their 70 us there with one scalar atomic per
-    // channel and block), so the count of operations per line is what matters — see also nn_grid_cap().
+    float* row = part + (size_t)blockIdx.x * ld + grp * V;
 #pragma unroll
-    for (int k = 0; k < V; k += 4)
-      asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(gb + grp * V + k), "f"(s[k]), "f"(s[k + 1]),
-                   "f"(s[k + 2]), "f"(s[k + 3]) : "memory");
+    for (int k = 0; k < V; k += 4) *reinterpret_cast<float4*>(row + k) = make_float4(s[k], s[k + 1], s[k + 2], s[k + 3]);
+  }
+}
+
+// dst[c] += sum of part[b * ld + c] over b < nrows, in a fixed order: a block takes 32 columns, its 8 warps the rows
+// b = warp (mod 8) in ascending order, and warp 0 adds the 8 sums up in warp order
+__global__ void __launch_bounds__(256) sum_rows_kernel(const float* __restrict__ part, float* __restrict__ dst, int nrows, int ld) {
+  __shared__ float sums[8][32];
+  const int cx = threadIdx.x & 31, g = threadIdx.x >> 5, c = blockIdx.x * 32 + cx;
+  float v = 0.f;
+  if (c < ld)
+    for (int b = g; b < nrows; b += 8) v += part[(size_t)b * ld + c];
+  sums[g][cx] = v;
+  __syncthreads();
+  if (g == 0 && c < ld) {
+    float t = sums[0][cx];
+#pragma unroll
+    for (int k = 1; k < 8; k++) t += sums[k][cx];
+    dst[c] += t;
   }
 }
 
@@ -67,7 +82,7 @@ __global__ void __launch_bounds__(256) relu_bwd_bias_grad_kernel(const T* __rest
   for (int k = 0; k < V; k++) acc[k] = 0.f;
   relu_bwd_thread<T, 4>(gy, y, gz, rows, cvec, blockDim.x / cvec, threadIdx.x % cvec, threadIdx.x / cvec, blockIdx.x,
                         gridDim.x, acc);
-  reduce_bias_grad<V>(acc, gb, cvec, smem);
+  reduce_bias_grad<V>(acc, gb, cvec * V, cvec, smem);
 }
 
 // ---- p = maxpool2x2(relu(z + b)) with a 1-byte index per element ---------------------------------
@@ -91,7 +106,7 @@ __global__ void __launch_bounds__(256) pool_relu_bwd_bias_grad_kernel(const T* _
   for (int k = 0; k < V; k++) acc[k] = 0.f;
   pool_relu_bwd_thread<T, 4>(gp, idx, gz, N, H, W, cvec, blockDim.x / cvec, threadIdx.x % cvec, threadIdx.x / cvec,
                              blockIdx.x, gridDim.x, acc);
-  reduce_bias_grad<V>(acc, gb, cvec, smem);
+  reduce_bias_grad<V>(acc, gb, cvec * V, cvec, smem);
 }
 
 // ---- BatchNorm (training) + ReLU + residual, four kernels (see nn_body.cuh) ------------------------------------
@@ -111,9 +126,9 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const T* __restrict__ z, 
   for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
   bn_stats_thread<T, 4>(z, rows, cvec, blockDim.x / cvec, threadIdx.x % cvec, threadIdx.x / cvec, blockIdx.x, gridDim.x, acc);
   const int C = cvec * V;
-  reduce_bias_grad<V>(acc, stats, cvec, smem);          // sum
+  reduce_bias_grad<V>(acc, stats, 2 * C, cvec, smem);          // sum
   __syncthreads();
-  reduce_bias_grad<V>(acc + V, stats + C, cvec, smem);  // sum of squares
+  reduce_bias_grad<V>(acc + V, stats + C, 2 * C, cvec, smem);  // sum of squares
 }
 
 // y = relu?(bn(z) (+ res)); block 0 also updates the running statistics (unbiased variance, PyTorch semantics)
@@ -157,9 +172,9 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const T* __restrict_
 #pragma unroll
   for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
   bn_bwd_reduce_thread<T, 2>(gy, y, z, rows, cvec, blockDim.x / cvec, grp, trow, blockIdx.x, gridDim.x, mean, invstd, relu != 0, acc);
-  reduce_bias_grad<V>(acc, gsum, cvec, smem);            // s1 = sum dy
+  reduce_bias_grad<V>(acc, gsum, 2 * C, cvec, smem);            // s1 = sum dy
   __syncthreads();
-  reduce_bias_grad<V>(acc + V, gsum + C, cvec, smem);    // s2 = sum dy * xhat
+  reduce_bias_grad<V>(acc + V, gsum + C, 2 * C, cvec, smem);    // s2 = sum dy * xhat
 }
 
 // gz, gres, and (block 0) the parameter gradients dgamma = s2, dbeta = s1
@@ -198,35 +213,54 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__
 
 using namespace bnet::nn;
 
-// Blocks of the column-reducing kernels (bias gradients, BatchNorm sums): every block ends with C/4 vector atomics on the
-// same 4*C bytes, and those serialise per cache line — so these kernels run as FEW resident blocks as still saturate HBM
-// (2 per SM x 256 threads x 8 x 16-byte loads in flight = 64 KiB per SM) and walk the rows in a loop.
-// BNET_NN_BLOCKS_PER_SM overrides (measured sweep: profiles/README.md).
+// SMs of the current device; 132 (H100 SXM) when there is none to ask
+static int sm_count() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0)
+      return v;
+    (void)cudaGetLastError();
+    return 132;
+  }();
+  return n;
+}
+
 static int nn_grid_cap() {
   static const int cap = [] {
     long long v = bnet::env_int("NN_BLOCKS_PER_SM", 2);
     if (v < 1) v = 1;
     if (v > 16) v = 16;
-    return (int)v * 148;
+    return (int)v * sm_count();
   }();
   return cap;
 }
 
+// dst[0 .. ld) += the `rows` partial rows the reduce kernel left in `part`
+static int finish_rows(const float* part, float* dst, int rows, int ld, cudaStream_t st) {
+  if (cudaGetLastError() != cudaSuccess) return -2;
+  sum_rows_kernel<<<(ld + 31) / 32, 256, 0, st>>>(part, dst, rows, ld);
+  return cudaGetLastError() == cudaSuccess ? 1 : -2;
+}
+
+// Rows of the workspace `part` the reduce entry points below may use: the caller passes part with at least this many rows
+// of C (bias gradients) or 2 C (BatchNorm sums) floats, e.g. a tensor allocated on the stream of the call.
+BNET_API int bnet_nn_partial_rows(void) { return nn_grid_cap(); }
+
 // dtype: 0 = f32, 1 = bf16 (same codes as bnet_coll.h).  All tensors NHWC-contiguous, C % vec == 0.
-// Return 1 (kernels launched) or <0.
+// Return 1 (the fused pass was launched) or <0.
 BNET_API int bnet_nn_bias_relu(void* z, const void* bias, long long rows, int C, int dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int V = dtype == 1 ? 8 : 4;
   if (C % V) return -1;
   size_t nvec = (size_t)rows * C / V;
-  int grid = (int)((nvec + 255) / 256 < 148 * 16 ? (nvec + 255) / 256 : 148 * 16);
+  int grid = (int)((nvec + 255) / 256 < sm_count() * 16 ? (nvec + 255) / 256 : sm_count() * 16);
   if (grid < 1) grid = 1;
   if (dtype == 1) bias_relu_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((__nv_bfloat16*)z, (const __nv_bfloat16*)bias, nvec, C / V);
   else bias_relu_kernel<float><<<grid, 256, 0, st>>>((float*)z, (const float*)bias, nvec, C / V);
   return cudaGetLastError() == cudaSuccess ? 1 : -2;
 }
 
-BNET_API int bnet_nn_relu_bwd_bias_grad(const void* gy, const void* y, void* gz, float* gb, long long rows, int C, int dtype,
+BNET_API int bnet_nn_relu_bwd_bias_grad(const void* gy, const void* y, void* gz, float* gb, float* part, long long rows, int C, int dtype,
                                         void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int V = dtype == 1 ? 8 : 4;
@@ -234,17 +268,18 @@ BNET_API int bnet_nn_relu_bwd_bias_grad(const void* gy, const void* y, void* gz,
   const int cvec = C / V;
   const int threads = (256 / cvec) * cvec;
   const int rpb = threads / cvec;
-  // at least 8 rows per thread before another block is worth its C atomics (small late layers: few rows, many channels)
+  // at least 8 rows per thread before another block is worth its partial row (small late layers: few rows, many channels)
   long long want = (rows + 8LL * rpb - 1) / (8LL * rpb);
   int grid = (int)(want < nn_grid_cap() ? want : nn_grid_cap());
   if (grid < 1) grid = 1;
+  if (!part) return -1;
   size_t smem = (size_t)threads * V * sizeof(float);
   if (dtype == 1)
     relu_bwd_bias_grad_kernel<__nv_bfloat16><<<grid, threads, smem, st>>>((const __nv_bfloat16*)gy, (const __nv_bfloat16*)y,
-                                                                       (__nv_bfloat16*)gz, gb, (size_t)rows, cvec);
+                                                                       (__nv_bfloat16*)gz, part, (size_t)rows, cvec);
   else
-    relu_bwd_bias_grad_kernel<float><<<grid, threads, smem, st>>>((const float*)gy, (const float*)y, (float*)gz, gb, (size_t)rows, cvec);
-  return cudaGetLastError() == cudaSuccess ? 1 : -2;
+    relu_bwd_bias_grad_kernel<float><<<grid, threads, smem, st>>>((const float*)gy, (const float*)y, (float*)gz, part, (size_t)rows, cvec);
+  return finish_rows(part, gb, grid, C, st);
 }
 
 BNET_API int bnet_nn_bias_relu_pool_fwd(const void* z, const void* bias, void* p, void* idx, int N, int H, int W, int C, int dtype,
@@ -253,7 +288,7 @@ BNET_API int bnet_nn_bias_relu_pool_fwd(const void* z, const void* bias, void* p
   const int V = dtype == 1 ? 8 : 4;
   if (C % V || (H & 1) || (W & 1)) return -1;
   size_t total = (size_t)N * (H / 2) * (W / 2) * (C / V);
-  int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  int grid = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
   if (grid < 1) grid = 1;
   if (dtype == 1)
     bias_relu_pool_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)z, (const __nv_bfloat16*)bias,
@@ -263,7 +298,7 @@ BNET_API int bnet_nn_bias_relu_pool_fwd(const void* z, const void* bias, void* p
   return cudaGetLastError() == cudaSuccess ? 1 : -2;
 }
 
-BNET_API int bnet_nn_pool_relu_bwd_bias_grad(const void* gp, const void* idx, void* gz, float* gb, int N, int H, int W, int C,
+BNET_API int bnet_nn_pool_relu_bwd_bias_grad(const void* gp, const void* idx, void* gz, float* gb, float* part, int N, int H, int W, int C,
                                              int dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int V = dtype == 1 ? 8 : 4;
@@ -272,17 +307,18 @@ BNET_API int bnet_nn_pool_relu_bwd_bias_grad(const void* gp, const void* idx, vo
   const int threads = (256 / cvec) * cvec;
   const int rpb = threads / cvec;
   long long rows = (long long)N * (H / 2) * (W / 2);
-  // at least 8 rows per thread before another block is worth its C atomics (small late layers: few rows, many channels)
+  // at least 8 rows per thread before another block is worth its partial row (small late layers: few rows, many channels)
   long long want = (rows + 8LL * rpb - 1) / (8LL * rpb);
   int grid = (int)(want < nn_grid_cap() ? want : nn_grid_cap());
   if (grid < 1) grid = 1;
+  if (!part) return -1;
   size_t smem = (size_t)threads * V * sizeof(float);
   if (dtype == 1)
     pool_relu_bwd_bias_grad_kernel<__nv_bfloat16><<<grid, threads, smem, st>>>((const __nv_bfloat16*)gp, (const uint8_t*)idx,
-                                                                            (__nv_bfloat16*)gz, gb, N, H, W, cvec);
+                                                                            (__nv_bfloat16*)gz, part, N, H, W, cvec);
   else
-    pool_relu_bwd_bias_grad_kernel<float><<<grid, threads, smem, st>>>((const float*)gp, (const uint8_t*)idx, (float*)gz, gb, N, H, W, cvec);
-  return cudaGetLastError() == cudaSuccess ? 1 : -2;
+    pool_relu_bwd_bias_grad_kernel<float><<<grid, threads, smem, st>>>((const float*)gp, (const uint8_t*)idx, (float*)gz, part, N, H, W, cvec);
+  return finish_rows(part, gb, grid, C, st);
 }
 
 
@@ -294,10 +330,10 @@ RowGrid row_grid(long long rows, int cvec, int V, int accs) {
   RowGrid g;
   g.threads = (256 / cvec) * cvec;
   const int rpb = g.threads / cvec;
-  // at least 8 rows per thread before another block is worth its C atomics (small late layers: few rows, many channels)
+  // at least 8 rows per thread before another block is worth its partial row (small late layers: few rows, many channels)
   long long want = (rows + 8LL * rpb - 1) / (8LL * rpb);
-  // the element-wise kernels (accs == 0) have no atomics at their end: they keep the larger grid
-  const int cap = accs ? nn_grid_cap() : 148 * 8;
+  // the element-wise kernels (accs == 0) leave no partial rows: they keep the larger grid
+  const int cap = accs ? nn_grid_cap() : sm_count() * 8;
   g.grid = (int)(want < cap ? want : cap);
   if (g.grid < 1) g.grid = 1;
   g.smem = (size_t)g.threads * V * sizeof(float) * (accs ? 1 : 0);
@@ -305,14 +341,15 @@ RowGrid row_grid(long long rows, int cvec, int V, int accs) {
 }
 }  // namespace
 
-BNET_API int bnet_nn_bn_stats(const void* z, float* stats, long long rows, int C, int dtype, void* stream) {
+BNET_API int bnet_nn_bn_stats(const void* z, float* stats, float* part, long long rows, int C, int dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int V = dtype == 1 ? 8 : 4;
   if (C % V || C / V > 256 || rows < 1) return -1;
   const RowGrid g = row_grid(rows, C / V, V, 1);
-  if (dtype == 1) bn_stats_kernel<__nv_bfloat16><<<g.grid, g.threads, g.smem, st>>>((const __nv_bfloat16*)z, stats, (size_t)rows, C / V);
-  else bn_stats_kernel<float><<<g.grid, g.threads, g.smem, st>>>((const float*)z, stats, (size_t)rows, C / V);
-  return cudaGetLastError() == cudaSuccess ? 1 : -2;
+  if (!part) return -1;
+  if (dtype == 1) bn_stats_kernel<__nv_bfloat16><<<g.grid, g.threads, g.smem, st>>>((const __nv_bfloat16*)z, part, (size_t)rows, C / V);
+  else bn_stats_kernel<float><<<g.grid, g.threads, g.smem, st>>>((const float*)z, part, (size_t)rows, C / V);
+  return finish_rows(part, stats, g.grid, 2 * C, st);
 }
 
 BNET_API int bnet_nn_bn_apply(const void* z, const void* res, void* y, const float* stats, const void* gamma, const void* beta,
@@ -334,19 +371,20 @@ BNET_API int bnet_nn_bn_apply(const void* z, const void* res, void* y, const flo
   return cudaGetLastError() == cudaSuccess ? 1 : -2;
 }
 
-BNET_API int bnet_nn_bn_bwd_reduce(const void* gy, const void* y, const void* z, const float* stats, float* gsum, long long rows,
+BNET_API int bnet_nn_bn_bwd_reduce(const void* gy, const void* y, const void* z, const float* stats, float* gsum, float* part, long long rows,
                                    int C, float eps, int relu, int dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int V = dtype == 1 ? 8 : 4;
   if (C % V || C / V > 256 || rows < 1) return -1;
   const RowGrid g = row_grid(rows, C / V, V, 1);
+  if (!part) return -1;
   if (dtype == 1)
     bn_bwd_reduce_kernel<__nv_bfloat16><<<g.grid, g.threads, g.smem, st>>>((const __nv_bfloat16*)gy, (const __nv_bfloat16*)y,
-                                                                          (const __nv_bfloat16*)z, stats, gsum, (size_t)rows, C / V, eps, relu);
+                                                                          (const __nv_bfloat16*)z, stats, part, (size_t)rows, C / V, eps, relu);
   else
-    bn_bwd_reduce_kernel<float><<<g.grid, g.threads, g.smem, st>>>((const float*)gy, (const float*)y, (const float*)z, stats, gsum,
+    bn_bwd_reduce_kernel<float><<<g.grid, g.threads, g.smem, st>>>((const float*)gy, (const float*)y, (const float*)z, stats, part,
                                                                   (size_t)rows, C / V, eps, relu);
-  return cudaGetLastError() == cudaSuccess ? 1 : -2;
+  return finish_rows(part, gsum, g.grid, 2 * C, st);
 }
 
 BNET_API int bnet_nn_bn_bwd_apply(const void* gy, const void* y, const void* z, void* gz, void* gres, const float* stats,

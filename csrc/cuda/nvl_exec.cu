@@ -1,4 +1,4 @@
-// sm_100a copy/reduce executor behind the NVLink transport's isend (K1, K4, K5, K7,
+// sm_90a copy/reduce executor behind the NVLink transport's isend (K1, K4, K5, K7,
 // K8 of SURVEY.md §2.6).
 //
 // One "device stream" = one thread-block cluster running a semi-persistent kernel
@@ -132,7 +132,7 @@ bnet_nvl_stream_kernel(ClusterQ* q, uint64_t idle_ns, uint64_t first_idle_ns, co
   uint64_t head = q->head;            // same value in every CTA of the cluster
   uint64_t last_work = ptx::globaltimer();
   // armed at connection setup: wait longer for the FIRST job so that it needs no launch on the
-  // data path (a launch can be held up by a cudaFree elsewhere in the process: profiles/blocking_calls.txt)
+  // data path (a launch can be held up by a cudaFree elsewhere in the process: tools/blocking_calls_probe.py)
   uint64_t idle_limit = first_idle_ns > idle_ns ? first_idle_ns : idle_ns;
   for (;;) {
     // ---- leader: wait for the next descriptor, publish it to every CTA of the cluster
@@ -582,7 +582,7 @@ Exec* get_exec(int dev) {
   }
   if (good) {
     // CUDA loads kernels lazily, and loading one may need to synchronise the context
-    // (measured: profiles/blocking_calls.txt — a first launch waits for every running kernel).
+    // (tools/blocking_calls_probe.py: a first launch waits for every running kernel).
     // On the data path that is a dead-lock: the NCCL kernel that is running is waiting for this
     // very transfer.  So load AND run every kernel once now, in the setup phase.
     cudaFuncAttributes fa;

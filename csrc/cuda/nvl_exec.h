@@ -1,5 +1,5 @@
 // Device copy executor used by the NVLink transport: moves a registered buffer
-// into the peer GPU's buffer with sm_100a kernels (K1/K8 in SURVEY.md §2.6).
+// into the peer GPU's buffer with sm_90a kernels (K1/K8 in SURVEY.md §2.6).
 //
 // A transfer is split into chunks of max(ceil(n/nclusters), MIN_CHUNKSIZE) bytes —
 // the same rule the reference uses to stripe a message over its TCP streams

@@ -1,4 +1,4 @@
-// Inline-PTX helpers for the sm_100a kernels (memory-model loads/stores, vector
+// Inline-PTX helpers for the sm_90a kernels (memory-model loads/stores, vector
 // reductions, clusters/DSMEM, mbarrier + bulk async copies, NVLS multimem).
 #pragma once
 #include <cuda_runtime.h>

@@ -1,8 +1,8 @@
-// Index logic of the tcgen05 linear kernel (csrc/cuda/tc_gemm.cu) as plain __host__ __device__ code: how a problem becomes
+// Index logic of the wgmma linear kernel (csrc/cuda/tc_gemm.cu) as plain __host__ __device__ code: how a problem becomes
 // tiles, tensor maps and kernel arguments, which TMA boxes a k-block needs, where an accumulator element goes.  The kernel
 // calls these functions; csrc/tests/tc_emu_test.cc compiles the same header with g++ and runs every mode of the kernel
 // (both orientations, MN-major operands, split-K, cross-rank adds, reduce-scatter, all-gather) on an emulated TMA / MMA /
-// TMEM — everything except the hardware's descriptor semantics, which csrc/tests/tc_desc_test.cc pins against CuTe.
+// accumulator — everything except the hardware's descriptor semantics, which csrc/tests/tc_desc_test.cc pins against CuTe.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -19,13 +19,19 @@
 namespace bnet {
 namespace tc {
 
-constexpr int kBM = 128;               // UMMA M: one accumulator row per TMEM lane
+constexpr int kBM = 128;               // accumulator rows of a tile: two consumer warpgroups x wgmma M = 64
 constexpr int kBK = 64;                // 64 bf16 = 128 bytes = one swizzle-128B row
-constexpr int kUmmaK = 16;             // fixed for 16-bit inputs
+constexpr int kMmaK = 16;              // wgmma K, fixed for 16-bit inputs
 constexpr int kABytes = kBM * kBK * 2; // lane-operand bytes per stage
 constexpr int kAtomBytes = 64 * kBK * 2; // one [64 x 64] box of an MN-major operand
+constexpr int kEpiPitch = 40;          // floats per row of a warp's epilogue scratch (16 rows x 32 columns)
+constexpr int kEpiScratchBytes = 8 * 16 * kEpiPitch * 4;   // the 8 consumer warps' scratch
 
 BNET_TC_HD constexpr int stages_for(int bn) { return bn <= 64 ? 6 : (bn <= 128 ? 5 : 4); }
+// dynamic shared memory of a launch: the stage ring + alignment slack + epilogue scratch + 2 mbarriers per stage + fix-up slot
+BNET_TC_HD constexpr int smem_bytes_for(int stages, int bn) {
+  return stages * (kABytes + bn * kBK * 2) + 1024 + kEpiScratchBytes + 2 * stages * 8 + 16;
+}
 
 // ---- bf16 without cuda_bf16.h (the header is also compiled by g++)
 BNET_TC_HD float bf16_to_f32(uint16_t v) {
@@ -80,7 +86,9 @@ struct TcArgs {
                              //      THAT rank's output only, at local row m % scatter_rows (reduce-scatter epilogue)
   int* err;
   // split-K with the finish fused into the kernel ("fix-up"): outs[0] is an fp32 workspace that is all zero on entry; the
-  // K slices add their partial tiles into it, count themselves in fix_counters[tile], and the slice that arrives last
+  // K slices add their partial tiles into it in slice order (slice z waits until fix_counters[tile] == z: the same sums on
+  // every run; fix_counters[n_tiles] hands out the slices' positions), count themselves in fix_counters[tile], and the slice
+  // that arrives last
   // reads the sums back (they sit in L2), applies bias / activation, writes the bf16 result and re-zeroes what it read —
   // one launch, no memset, no separate epilogue pass.  fix_out == nullptr: plain reduce mode.
   void* fix_out;
@@ -97,12 +105,12 @@ struct Operand { const void* ptr; int rows; int ld; int mn; };
 struct MapDesc { const void* ptr; long long dim0, dim1; long long pitch_elems; int box0, box1; };
 
 // ---- tiling --------------------------------------------------------------------------------------------------------------
-// D[batch, feat]: `batch_rows` decides the orientation (<= 64: features ride the 128 TMEM lanes, "swap").
+// D[batch, feat]: `batch_rows` decides the orientation (<= 64: features ride the 128 accumulator rows, "swap").
 inline int plan_gemm(int batch_rows, int feat_rows, int red, int reduce, int splits, int sm_count, BnetTcPlan* p) {
   const int M = batch_rows, N = feat_rows;
   p->swap = M <= 64 ? 1 : 0;
   p->bn = p->swap ? (M <= 32 ? 32 : 64) : 128;
-  // 128 x 256 tiles (the whole TMEM: 2 x 256 accumulator columns) once they still fill every SM: half the MMA issues and
+  // 128 x 256 tiles (128 accumulator registers per consumer thread) once they still fill every SM: half the MMA issues and
   // 1.5x the arithmetic intensity per shared-memory byte of a 128 x 128 tile
   if (!p->swap && (long long)((N + 255) / 256) * ((M + kBM - 1) / kBM) >= sm_count) p->bn = 256;
   p->stages = stages_for(p->bn);
@@ -114,8 +122,7 @@ inline int plan_gemm(int batch_rows, int feat_rows, int red, int reduce, int spl
   if (z > p->k_blocks) z = p->k_blocks;
   p->k_per_split = (p->k_blocks + z - 1) / z;
   p->grid_z = (p->k_blocks + p->k_per_split - 1) / p->k_per_split;   // no empty slices
-  // tiles + alignment slack + (2 * stages + 4) mbarriers + the TMEM address slot
-  p->smem_bytes = p->stages * (kABytes + p->bn * kBK * 2) + 1024 + (2 * p->stages + 4) * 8 + 16;
+  p->smem_bytes = smem_bytes_for(p->stages, p->bn);
   if (p->grid_z > 65535 || (long long)p->grid_x * p->grid_y > 0x7fffffffLL) return -1;
   // persistent once there are more tiles than SMs: one CTA per SM (shared memory allows no second one anyway)
   const int n_tiles = p->grid_x * p->grid_y;
@@ -332,7 +339,7 @@ inline const char* setup_conv(const void* x, const void* w, const void* bias, vo
   p.grid_z = 1;
   p.k_blocks = 9 * g.cpb;
   p.k_per_split = p.k_blocks;
-  p.smem_bytes = p.stages * (kABytes + bn_cols * kBK * 2) + 1024 + (2 * p.stages + 4) * 8 + 16;
+  p.smem_bytes = smem_bytes_for(p.stages, bn_cols);
   const long long n_tiles = (long long)p.grid_x * p.grid_y;
   if (n_tiles > 0x7fffffffLL) return "too many tiles";
   p.ctas = n_tiles < sm_count ? (int)n_tiles : sm_count;
@@ -371,7 +378,7 @@ inline const char* setup_conv(const void* x, const void* w, const void* bias, vo
 // A box lands in shared memory as [64 pixel rows x 128 bytes], exactly the [64 reduction rows x 64 MN elements] atom the
 // MN-major shared-memory descriptor describes (the layout the linear layer's dW = gY^T . X already uses).  Padding, ragged
 // patches, channels past Cout and columns past 9 * Cin are all the TMA unit's zero fill.  The pixel blocks are split over
-// grid.z (split-K with the fix-up: TcArgs::fix_out), because Cout x 9 Cin alone rarely fills 148 SMs.
+// grid.z (split-K with the fix-up: TcArgs::fix_out), because Cout x 9 Cin alone rarely fills 132 SMs.
 template <int BN, class FA, class FB>
 BNET_TC_HD void wgrad_stage_loads(const TcArgs& args, const TileCoord& c, int kb, FA&& lda, FB&& ldb) {
   const ConvGeom& g = args.conv;
@@ -408,8 +415,9 @@ struct WgradProblem {
 
 // dw[Cout][3][3][Cin] (bf16) = filter gradient of y = conv3x3(x, w), stride 1, pad 1; gy [N,H,W,Cout], x [N,H,W,Cin] NHWC bf16.
 // `ws`: fp32 [Cout][9 * Cin] workspace, `counters`: one int per output tile (>= wgrad_max_tiles), both all zero on entry and
-// left all zero.  splits <= 0: as many K slices as fill the SMs.  Pure: no CUDA calls.
-inline int wgrad_max_tiles(int Cin, int Cout) { return ((Cout + kBM - 1) / kBM) * ((9 * Cin + 127) / 128); }
+// left all zero.  splits <= 0: as many K slices as keep the SMs busy.  Pure: no CUDA calls.
+// (+ 1: the int after the tile counters is the fix-up's ticket, see tc_gemm.cu)
+inline int wgrad_max_tiles(int Cin, int Cout) { return ((Cout + kBM - 1) / kBM) * ((9 * Cin + 127) / 128) + 1; }
 
 // fixup == 0: plain reduce mode — the slices only ADD into `ws` (fp32 [Cout][9 Cin], zero on entry) and the caller converts
 // it to bf16 and clears it afterwards (two small passes); the fall-back when the in-kernel finish cannot be trusted.
@@ -452,12 +460,26 @@ inline const char* setup_conv_wgrad(const void* gy, const void* x, float* ws, vo
   p.grid_y = tiles_a;
   p.k_blocks = (int)kblocks;
   const int n_tiles = tiles_a * tiles_b;
-  int z = splits > 0 ? splits : (sm_count / n_tiles > 0 ? sm_count / n_tiles : 1);
+  int z = splits;
+  if (z <= 0) {
+    // automatic: a slice runs sm_count / z persistent CTAs, so z slices finish after ceil(n_tiles / (sm_count / z)) tile
+    // passes of 1 / z of the pixels each.  Take the smallest z within 5 % of the best such time — every further slice
+    // adds its partial tiles into the workspace once more.
+    const long long zmax = kblocks < sm_count ? kblocks : sm_count;
+    auto cost = [&](long long zz) {
+      const long long per = sm_count / zz > 0 ? sm_count / zz : 1;
+      return double((n_tiles + per - 1) / per) / double(zz);
+    };
+    double best = cost(1);
+    for (long long zz = 2; zz <= zmax; zz++) best = cost(zz) < best ? cost(zz) : best;
+    z = 1;
+    while (z < zmax && cost(z) > best * 1.05) z++;
+  }
   if (z > p.k_blocks) z = p.k_blocks;
   if (z > 65535) z = 65535;
   p.k_per_split = (p.k_blocks + z - 1) / z;
   p.grid_z = (p.k_blocks + p.k_per_split - 1) / p.k_per_split;      // no empty slices
-  p.smem_bytes = p.stages * (kABytes + bn_cols * kBK * 2) + 1024 + (2 * p.stages + 4) * 8 + 16;
+  p.smem_bytes = smem_bytes_for(p.stages, bn_cols);
   const int per_slice = sm_count / p.grid_z > 0 ? sm_count / p.grid_z : 1;
   p.ctas = n_tiles < per_slice ? n_tiles : per_slice;
   a.rows_a = Cout;

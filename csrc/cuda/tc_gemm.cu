@@ -1,39 +1,37 @@
-// Tensor-core linear layer for sm_100a: TMA -> shared memory -> tcgen05.mma -> TMEM -> fused epilogue.
+// Tensor-core linear layer for sm_90a: TMA -> shared memory -> wgmma (fp32 accumulator in registers) -> fused epilogue.
 //
-//   D[i, j] = sum_k A[i, k] * B[j, k]        A: "lane" operand, 128 rows per tile (one per TMEM lane)
+//   D[i, j] = sum_k A[i, k] * B[j, k]        A: "lane" operand, 128 rows per tile (64 per consumer warpgroup)
 //                                            B: "column" operand, BN rows per tile (the MMA N dimension)
 //
 // Forward: both operands are K-major bf16 matrices (a torch Linear's activation [M,K] and weight [N,K] as they are), so
 // either can take either role: with a large batch x is A and w is B; with a small batch (M <= 64) the roles swap so that
-// the 128 TMEM lanes are filled by output features instead of 3/4 padding rows.
+// the 128 accumulator rows are filled by output features instead of 3/4 padding rows.
 // Backward: dX = gY . W reduces over N and dW = gY^T . X reduces over M, so W, gY and X appear with the reduction
 // dimension OUTER ("MN-major" operands).  Those are staged as [64 reduction rows x 64 MN elements] TMA boxes (one per 64
-// MN elements of the tile, 8 KiB each) and described to the MMA with the MN-major form of the shared-memory descriptor;
-// no transposed copy of any tensor is ever made.
+// MN elements of the tile, 8 KiB each) and handed to wgmma with the transpose bit and the MN-major form of the
+// shared-memory descriptor; no transposed copy of any tensor is ever made.
 //
-// Persistent CTAs (one per SM once there are more tiles than SMs), 6 warps, warp-specialised (guide "Anatomy of a
-// Blackwell GEMM kernel"); the ring of shared-memory stages runs through tile boundaries:
-//   warp 0, one lane   TMA producer: per stage one [128 x 64] lane box and one [BN x 64] column box (K-major operands) or
-//                      [64 x 64] boxes per 64 MN elements (MN-major operands), 128-byte swizzle, completion on the
-//                      stage's `full` mbarrier; a gathered batch operand is loaded from the owning rank's tensor map
-//   warp 1             allocates 2 x BN TMEM columns (two accumulator stages); one lane issues 4 tcgen05.mma (K = 16
-//                      each) per stage and tcgen05.commit's the stage's `empty` mbarrier; after a tile's last K block it
-//                      commits `acc_full[stage]`, and before reusing a stage it waits for `acc_empty[stage]`
-//   warps 2-5          epilogue: tcgen05.ld 32 lanes x 16 columns at a time -> bias / ReLU -> bf16 store, or (reduce
-//                      mode) fp32 adds into every rank's output — multimem.red through the NVSwitch multicast mapping
-//                      or red.global per peer — or into the owner's output only (reduce-scatter); arrives on
-//                      `acc_empty[stage]` as soon as the accumulator is in registers.  Warp w may only touch TMEM
-//                      lanes 32*(w%4) .. +31.
+// Persistent CTAs (one per SM once there are more tiles than SMs), 3 warpgroups, warp-specialised; the ring of
+// shared-memory stages runs through tile boundaries:
+//   warpgroup 0, one lane  TMA producer: per stage one [128 x 64] lane box and one [BN x 64] column box (K-major operands) or
+//                          [64 x 64] boxes per 64 MN elements (MN-major operands), 128-byte swizzle, completion on the
+//                          stage's `full` mbarrier; a gathered batch operand is loaded from the owning rank's tensor map
+//   warpgroups 1 and 2     consumers: warpgroup c owns accumulator rows 64c .. 64c+63 of the tile (BN / 2 fp32 registers per
+//                          thread).  Per stage it issues 4 wgmma.mma_async (m64 x BN x k16) and keeps one stage's group in
+//                          flight: once the previous group has completed, that stage goes back to the producer through its
+//                          `empty` mbarrier (one arrive per warpgroup).  After the tile's last K block each warp passes its
+//                          16 x BN accumulator through a shared-memory scratch, 16 x 32 at a time, so that every thread holds
+//                          16 consecutive columns of one row -> bias / ReLU -> bf16 store, or (reduce mode) fp32 adds into
+//                          every rank's output — multimem.red through the NVSwitch multicast mapping or red.global per
+//                          peer — or into the owner's output only (reduce-scatter).  Meanwhile the producer already fills
+//                          the ring with the next tile's stages.
 // The index logic (tiling, TMA coordinates, epilogue addressing) is csrc/cuda/tc_body.cuh, shared with the CPU
 // emulation test; the mbarrier protocol is mirrored by tests/test_tc_pipeline_model.py.
 //
 // Every mbarrier wait carries a watchdog (kWatchdogNs): a pipeline that stops — a descriptor the hardware rejects, a
 // lost TMA completion — sets *err and lets every role fall through to the teardown instead of hanging the GPU.
-//
-// STATUS: validated on B200 in round 2 (profiles/r2/tc_probe_1gpu.txt: every probe of tools/tc_probe.py, linear forward /
-// backward, split-K, GEMM + all-reduce, 3x3 convolution forward + input gradient); the convolution WEIGHT gradient
-// (kConv == 2) was written afterwards and has only run on the CPU emulation — ops/tc_conv.py therefore trusts it only after a
-// self-check in a child process on the GPU at hand.  Descriptor packing is unit-tested against CuTe (csrc/tests/tc_desc_test.cc).
+// ops/tc_linear.py and ops/tc_conv.py trust the kernels only after a self-check in a child process on the GPU at hand.
+// Descriptor packing is unit-tested against CuTe (csrc/tests/tc_desc_test.cc).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -55,36 +53,28 @@ namespace {
 using namespace bnet;
 using namespace bnet::tc;              // tile constants, TcArgs, plan / setup, per-tile index logic (tc_body.cuh)
 
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;          // producer warpgroup + two consumer warpgroups
 constexpr uint64_t kWatchdogNs = 2000000000ull;
 
 thread_local std::string g_err;
 
 // ------------------------------------------------------------------------------------------------ descriptors
-// Instruction descriptor, .kind::f16 (bit positions: cute/arch/mma_sm100_desc.hpp `InstrDescriptor`):
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   15 / 16 A / B major (0 = K-major)   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t instr_desc_bf16_f32(int m, int n, bool a_mn = false, bool b_mn = false) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(a_mn) << 15) | (uint32_t(b_mn) << 16) | (uint32_t(n >> 3) << 17) |
-         (uint32_t(m >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor of a K-major tile whose rows are 128 bytes, stored densely and swizzled by the
-// hardware in 8-row x 128-byte atoms (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B):
-//   [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major layouts; 1 like CuTe)
-//   [32,46) stride byte offset >> 4 = 1024 B between 8-row groups   [46,48) version = 1   [61,64) layout = 2 (SW128)
+// Shared-memory matrix descriptor of wgmma (bit positions: cute/arch/mma_sm90_desc.hpp `GmmaDescriptor`):
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4   [49,52) base offset
+//   [62,64) layout (1 = 128-byte swizzle)
+// K-major tile whose rows are 128 bytes, stored densely and swizzled by the hardware in 8-row x 128-byte atoms (what TMA
+// writes with CU_TENSOR_MAP_SWIZZLE_128B): leading byte offset unused (1 like CuTe), stride byte offset = 1024 B between
+// 8-row groups.  Every stage starts on a 1024-byte boundary, so the base offset is 0.
 __host__ __device__ constexpr uint64_t smem_desc_sw128(uint32_t smem_addr) {
-  return uint64_t((smem_addr >> 4) & 0x3FFF) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
+  return uint64_t((smem_addr >> 4) & 0x3FFF) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
 
 // The same for an MN-major tile staged as [64 reduction rows x 128 bytes] boxes, one per 64 MN elements, 8 KiB apart:
 //   leading byte offset = 8192 B between 64-element MN atoms, stride byte offset = 1024 B between 8-row reduction groups
-//   (CuTe: make_umma_desc<Major::MN> of tile_to_shape(Layout_MN_SW128_Atom<bf16>, (MN, 64), Step<_2,_1>) -> LBO 512, SBO 64).
+//   (CuTe: make_gmma_desc<Major::MN> of tile_to_shape(Layout_MN_SW128_Atom<bf16>, (MN, 64), Step<_2,_1>) -> LBO 512, SBO 64).
 // One K = 16 slice is two 8-row groups further: +2048 B.
 __host__ __device__ constexpr uint64_t smem_desc_sw128_mn(uint32_t smem_addr) {
-  return uint64_t((smem_addr >> 4) & 0x3FFF) | (uint64_t(8192 >> 4) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
+  return uint64_t((smem_addr >> 4) & 0x3FFF) | (uint64_t(8192 >> 4) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
 
 // ------------------------------------------------------------------------------------------------ PTX
@@ -114,6 +104,9 @@ __device__ __forceinline__ bool mbar_wait_wd(uint32_t bar, uint32_t parity, int*
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -127,35 +120,38 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" :: "l"(map) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// wgmma ordering: fence before the first MMA that touches registers written by ordinary instructions; commit the MMAs
+// issued so far as one group; wait until at most N groups are pending
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i]) :: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem] * B[smem]; accumulate == 0 overwrites D
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// true when any of the `count` threads arriving at named barrier `id` passes true
+__device__ __forceinline__ bool bar_any(int id, int count, bool v) {
+  uint32_t r;
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.or.pred q, %2, %3, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(r) : "r"(uint32_t(v)), "r"(id), "r"(count) : "memory");
+  return r != 0;
 }
-// mbarrier arrives once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory");
-}
-// this warp's 32 TMEM lanes x 16 consecutive fp32 columns: v[t] = D[lane, col + t]
-__device__ __forceinline__ void tmem_ld_16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// split-K fix-up: wait until `*turn` (the slices that have added their partial tile so far) reaches `mine`
+__device__ __forceinline__ void wait_turn(const int* turn, int mine, int* err) {
+  const uint64_t t0 = ptx::globaltimer();
+  while ((int)ptx::ld_acquire_sys_u32(reinterpret_cast<const volatile uint32_t*>(turn)) != mine) {
+    if (ptx::globaltimer() - t0 > kWatchdogNs) {
+      atomicCAS(err, 0, 3);
+      return;
+    }
+  }
 }
 __device__ __forceinline__ void multimem_red_add_f32(float* mc, float v) {
   asm volatile("multimem.red.relaxed.sys.global.add.f32 [%0], %1;" :: "l"(mc), "f"(v) : "memory");
@@ -164,6 +160,51 @@ __device__ __forceinline__ void multimem_red_add_v4_f32(float* mc, const float4&
   asm volatile("multimem.red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};"
                :: "l"(mc), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
+
+// D (m64 x N, fp32, the warpgroup's registers) (+)= A[smem] * B[smem]^T; TA / TB = 1: the operand is MN-major (transposed).
+// Register d[4 j + e] of thread (warp w, lane l) holds D[16 w + l / 4 + 8 (e / 2), 8 j + 2 (l % 4) + e % 2].
+template <int N, int TA, int TB>
+struct Wgmma;
+template <int TA, int TB>
+struct Wgmma<32, TA, TB> {
+  __device__ __forceinline__ static void mma(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<128, TA, TB> {
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<256, TA, TB> {
+  __device__ __forceinline__ static void mma(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
 
 // ------------------------------------------------------------------------------------------------ kernel
 // the epilogue's memory operations (tc_body.cuh::epilogue_chunk)
@@ -197,18 +238,14 @@ struct Smem {
   static constexpr int kStageBytes = kABytes + kBBytes;
 };
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory");
-}
-
 // kSwap:   false -> A = x (lane i = batch row m), B = w (column j = feature n); out[m, n] = out[i * ldo + j]
 //          true  -> A = w (lane i = feature n),   B = x (column j = batch row m); out[m, n] = out[j * ldo + i]
 // kReduce: fp32 adds into args.outs[] instead of a bf16 store
 //
 // Persistent over output tiles: CTA c takes tiles c, c + gridDim.x, ... (consecutive CTAs share the column operand's
 // block, so it is read from HBM once and from L2 afterwards).  The shared-memory ring runs straight through tile
-// boundaries, and the accumulator is double-buffered in TMEM (2 x BN columns): the epilogue of tile t drains one half
-// while the MMAs of tile t+1 fill the other.  With gridDim.x == n_tiles every CTA simply does one tile.
+// boundaries: while the consumers run a tile's epilogue, the producer fills the stages of the next tile.  With
+// gridDim.x == n_tiles every CTA simply does one tile.
 // kAMn / kBMn: the lane / column operand is MN-major (reduction dimension outer) instead of K-major
 // kConv: 1 = the lane operand is a 3x3 convolution's input patch, loaded as 4-D TMA boxes (tc_body.cuh::ConvGeom);
 //        2 = convolution weight gradient: BOTH operands are 4-D boxes of NHWC activations (gy on the lanes through
@@ -216,52 +253,57 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 template <int BN, int kStages, bool kSwap, bool kReduce, bool kAMn, bool kBMn, int kConv = 0>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_linear_kernel(const __grid_constant__ TcBatchMaps maps_batch, const __grid_constant__ CUtensorMap map_feat, const TcArgs args) {
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N for M = 128");
-  static_assert((BN & (BN - 1)) == 0 && BN >= 32, "TMEM allocations are powers of two >= 32 columns");
+  static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "wgmma N, in whole 32-column epilogue chunks");
   static_assert(!kBMn || BN % 64 == 0, "an MN-major operand is staged in 64-element atoms");
   static_assert(kConv != 1 || (!kSwap && !kAMn && !kReduce), "convolution: pixels ride the lanes, K-major patches, bf16 store");
   static_assert(kConv != 2 || (!kSwap && kAMn && kBMn && kReduce), "weight gradient: MN-major operands, split over pixel blocks");
-  constexpr uint32_t kTmemCols = 2 * BN;          // two accumulator stages
   extern __shared__ uint8_t smem_raw[];
   // swizzle-128B atoms must start on 1024-byte boundaries of the shared window
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* const tiles = smem_raw + (base - raw);
-  uint64_t* const bars = reinterpret_cast<uint64_t*>(tiles + kStages * Smem<BN>::kStageBytes);
+  float* const scratch = reinterpret_cast<float*>(tiles + kStages * Smem<BN>::kStageBytes);
+  uint64_t* const bars = reinterpret_cast<uint64_t*>(scratch + kEpiScratchBytes / 4);
   const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * kStages;
-  const uint32_t acc_full0 = empty0 + 8 * kStages, acc_empty0 = acc_full0 + 16;
-  uint32_t* const tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
-  uint32_t* const last_slot = tmem_slot + 1;      // split-K fix-up: "this CTA's slice was the last one of the tile"
+  uint32_t* const last_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages);   // split-K fix-up: "this CTA's slice was last"
+  uint32_t* const pos_slot = last_slot + 1;                                       // this CTA's (x, z) position, z * gridDim.x + x
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kb_begin = blockIdx.z * args.k_per_split;
-  const int kb_end = min(kb_begin + args.k_per_split, args.k_blocks);
-  const int nkb = kb_end - kb_begin;       // >= 1 by construction of the grid
+  const bool fix = kReduce && args.fix_out != nullptr;
 
   if (warp == 0 && lane == 0) {
+    if (fix) {
+      // serial split-K (slice z adds after slices 0 .. z-1, below): positions are handed out in the order the CTAs START, so a
+      // slice only ever waits for slices whose CTAs already run or are done, however the hardware dispatches the grid.  The
+      // ticket is the int after the tile counters; the CTA that takes the last one puts it back to 0 for the next launch.
+      uint32_t* ticket = reinterpret_cast<uint32_t*>(args.fix_counters + args.n_tiles);
+      const uint32_t v = atomicAdd(ticket, 1u);
+      if (v == gridDim.x * gridDim.z - 1) atomicExch(ticket, 0u);
+      *pos_slot = v;
+    } else {
+      *pos_slot = blockIdx.z * gridDim.x + blockIdx.x;
+    }
     tma_prefetch_desc(&maps_batch.m[0]);
     tma_prefetch_desc(&map_feat);
     for (int s = 0; s < kStages; s++) {
       ptx::mbar_init(bars + s, 1);               // full: the producer's arrive.expect_tx (+ TMA bytes)
-      ptx::mbar_init(bars + kStages + s, 1);     // empty: one tcgen05.commit
-    }
-    for (int s = 0; s < 2; s++) {
-      ptx::mbar_init(bars + 2 * kStages + s, 1);       // accumulator stage complete: one tcgen05.commit
-      ptx::mbar_init(bars + 2 * kStages + 2 + s, 128); // accumulator stage drained: every epilogue thread
+      ptx::mbar_init(bars + kStages + s, 2);     // empty: one arrive per consumer warpgroup
     }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), kTmemCols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  const int bx = (int)(*pos_slot % gridDim.x), bz = (int)(*pos_slot / gridDim.x);
+  const int kb_begin = bz * args.k_per_split;
+  const int kb_end = min(kb_begin + args.k_per_split, args.k_blocks);
+  const int nkb = kb_end - kb_begin;       // >= 1 by construction of the grid
 
-  if (warp == 0) {
-    if (lane == 0) {
+  // the producer warpgroup needs few registers, a consumer holds BN / 2 accumulators: hand the register file over
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0) {
       uint32_t g = 0;                              // k-blocks issued by this CTA so far (ring position)
       bool alive = true;
-      for (int t = blockIdx.x; t < args.n_tiles && alive; t += gridDim.x) {
+      for (int t = bx; t < args.n_tiles && alive; t += gridDim.x) {
         // the operand that is the batch rides the lanes (plain) or the columns (swapped); when it is gathered, the tile's
         // rows come from ONE rank's map, at a row offset inside that rank's shard (tc_body.cuh::tile_coord)
         const TileCoord tc = tile_coord<BN, kSwap>(args, t);
@@ -290,118 +332,131 @@ tc_linear_kernel(const __grid_constant__ TcBatchMaps maps_batch, const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = instr_desc_bf16_f32(kBM, BN, kAMn, kBMn);
-      // descriptor advance per K = 16 slice, in 16-byte units: 32 B along the swizzled row (K-major), or two 8-row groups
-      // = 2048 B (MN-major)
-      constexpr uint64_t kStepA = kAMn ? 2048 / 16 : kUmmaK * 2 / 16, kStepB = kBMn ? 2048 / 16 : kUmmaK * 2 / 16;
-      uint32_t g = 0, lt = 0;                      // ring position; tiles done by this CTA
-      bool alive = true;
-      for (int t = blockIdx.x; t < args.n_tiles && alive; t += gridDim.x, lt++) {
-        const uint32_t as = lt & 1, use = lt >> 1;
-        // the epilogue must have drained this accumulator stage (two tiles ago) before it is overwritten
-        if (use > 0 && !mbar_wait_wd(acc_empty0 + 8 * as, (use - 1) & 1, args.err, 2)) break;
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int i = 0; i < nkb; i++, g++) {
-          const uint32_t s = g % kStages;
-          alive = mbar_wait_wd(full0 + 8 * s, (g / kStages) & 1, args.err, 2);
-          if (!alive) break;
-          tc_fence_after_sync();
-          const uint32_t a_src = base + s * Smem<BN>::kStageBytes;
-          const uint64_t da = kAMn ? smem_desc_sw128_mn(a_src) : smem_desc_sw128(a_src);
-          const uint64_t db = kBMn ? smem_desc_sw128_mn(a_src + kABytes) : smem_desc_sw128(a_src + kABytes);
-#pragma unroll
-          for (int k = 0; k < kBK / kUmmaK; k++)
-            umma_bf16(tmem_d, da + uint64_t(k) * kStepA, db + uint64_t(k) * kStepB, idesc, (i | k) != 0 ? 1u : 0u);
-          umma_commit(empty0 + 8 * s);            // the stage may be refilled once these MMAs have read it
-        }
-        if (alive) umma_commit(acc_full0 + 8 * as);
-      }
-    }
   } else {
-    // ---- epilogue: 4 warps x 32 lanes = the tile's 128 accumulator rows
-    const int q = warp & 3;                        // the TMEM lane quarter this warp may read
-    const bool fix = kReduce && args.fix_out != nullptr;
-    const bool add_bias = args.bias != nullptr && (!kReduce || blockIdx.z == 0) && !fix;
-    uint32_t lt = 0;
-    for (int t = blockIdx.x; t < args.n_tiles; t += gridDim.x, lt++) {
-      const uint32_t as = lt & 1;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    // ---- consumers: warpgroup c = accumulator rows 64c .. 64c+63; warp wq of it = rows 16 wq .. 16 wq + 15 of those
+    const int c = (warp >> 2) - 1, wq = warp & 3;
+    const int ctid = threadIdx.x - 128;            // 0 .. 255 over both consumer warpgroups
+    const bool signal = (warp & 3) == 0 && lane == 0;
+    // descriptor advance per K = 16 slice, in 16-byte units: 32 B along the swizzled row (K-major), or two 8-row groups
+    // = 2048 B (MN-major).  Warpgroup c's half of the lane operand starts 64 rows (K-major) or one 64-element atom
+    // (MN-major) further — 8 KiB either way.
+    constexpr uint64_t kStepA = kAMn ? 2048 / 16 : kMmaK * 2 / 16, kStepB = kBMn ? 2048 / 16 : kMmaK * 2 / 16;
+    float* const scr = scratch + (warp - 4) * (16 * kEpiPitch);
+    const bool add_bias = args.bias != nullptr && (!kReduce || bz == 0) && !fix;
+    float acc[BN / 2];
+    uint32_t g = 0;
+    bool alive = true;
+    for (int t = bx; t < args.n_tiles; t += gridDim.x) {
+      for (int i = 0; i < nkb; i++, g++) {
+        const uint32_t s = g % kStages;
+        alive = mbar_wait_wd(full0 + 8 * s, (g / kStages) & 1, args.err, 2);
+        if (!alive) break;
+        const uint32_t a_src = base + s * Smem<BN>::kStageBytes;
+        const uint64_t da = kAMn ? smem_desc_sw128_mn(a_src + c * 8192) : smem_desc_sw128(a_src + c * 8192);
+        const uint64_t db = kBMn ? smem_desc_sw128_mn(a_src + kABytes) : smem_desc_sw128(a_src + kABytes);
+        wgmma_fence();
+        fence_regs(acc);
+#pragma unroll
+        for (int k = 0; k < kBK / kMmaK; k++)
+          Wgmma<BN, kAMn, kBMn>::mma(acc, da + uint64_t(k) * kStepA, db + uint64_t(k) * kStepB, (i | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        fence_regs(acc);
+        if (i > 0) {
+          wgmma_wait<1>();                           // the previous stage's MMAs have read their operands
+          if (signal) mbar_arrive(empty0 + 8 * ((g - 1) % kStages));
+        }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (alive && signal) mbar_arrive(empty0 + 8 * ((g - 1) % kStages));
+      // both warpgroups agree before anything that synchronises them (the fix-up below) can wait for a quitter
+      if (bar_any(1, 256, !alive)) break;
+
       TileCoord tc = tile_coord<BN, kSwap>(args, t);
-      int i_glob = tc.a_row0 + q * 32 + lane;         // row of the lane operand this thread owns
+      ConvTile ct{};
       if constexpr (kConv == 1) {
-        // the lane is a pixel of the tile's patch: its row in the [N*H*W, Cout] output, or "past the end" outside the image
-        const ConvTile ct = conv_tile<BN>(args, t);
-        const long long row = conv_out_row(args, ct, q * 32 + lane);
-        i_glob = row < 0 ? args.rows_a : (int)row;
+        ct = conv_tile<BN>(args, t);
         tc.b_row0 = ct.b_row0;
       }
-      if (!mbar_wait_wd(acc_full0 + 8 * as, (lt >> 1) & 1, args.err, 3)) break;
-      tc_fence_after_sync();
-      const uint32_t tmem_d = tmem_base + as * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN / 16; c++) {
-        uint32_t v[16];
-        __syncwarp();                                 // tcgen05.ld is .sync.aligned: reconverge after the guarded stores
-        tmem_ld_16(tmem_d + (uint32_t(q * 32) << 16) + uint32_t(c * 16), v);
-        if (c == BN / 16 - 1) {
-          // the whole accumulator stage is in registers: hand it back to the MMA warp before the stores
-          tc_fence_before_sync();
-          mbar_arrive(acc_empty0 + 8 * as);
+      // ---- epilogue, 32 accumulator columns at a time: the warp's fragment goes to its scratch (row pitch kEpiPitch
+      //      floats keeps the float2 stores free of bank conflicts), then lane l takes row l % 16,
+      //      columns 16 (l / 16) .. +15
+      const int r_own = lane & 15, h_own = lane >> 4;
+      const int i_local = 64 * c + 16 * wq + r_own;     // row of the tile this thread finishes
+      int i_glob = tc.a_row0 + i_local;
+      if constexpr (kConv == 1) {
+        // the row is a pixel of the tile's patch: its row in the [N*H*W, Cout] output, or "past the end" outside the image
+        const long long row = conv_out_row(args, ct, i_local);
+        i_glob = row < 0 ? args.rows_a : (int)row;
+      }
+      if constexpr (kReduce) {
+        if (fix) {
+          // serial split-K: slice z adds its partial tile only after slices 0 .. z-1 have added theirs, so every element is
+          // summed in the same order on every run (the counter is the one the fix-up below advances)
+          if (ctid == 0) wait_turn(args.fix_counters + t, bz, args.err);
+          asm volatile("bar.sync 1, 256;" ::: "memory");
         }
-        float acc[16];
+      }
 #pragma unroll
-        for (int u = 0; u < 16; u++) acc[u] = __uint_as_float(v[u]);
-        epilogue_chunk<kSwap, kReduce>(args, i_glob, tc.b_row0 + c * 16, acc, add_bias, DeviceOut{});
+      for (int cc = 0; cc < BN / 32; cc++) {
+        __syncwarp();
+#pragma unroll
+        for (int jj = 0; jj < 4; jj++) {
+          const int j = 4 * cc + jj, col = 8 * jj + 2 * (lane & 3), row = lane >> 2;
+          *reinterpret_cast<float2*>(scr + row * kEpiPitch + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(scr + (row + 8) * kEpiPitch + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        __syncwarp();
+        float v[16];
+#pragma unroll
+        for (int u = 0; u < 16; u += 4) {
+          const float4 x = *reinterpret_cast<const float4*>(scr + r_own * kEpiPitch + 16 * h_own + u);
+          v[u] = x.x; v[u + 1] = x.y; v[u + 2] = x.z; v[u + 3] = x.w;
+        }
+        epilogue_chunk<kSwap, kReduce>(args, i_glob, tc.b_row0 + 32 * cc + 16 * h_own, v, add_bias, DeviceOut{});
       }
       if constexpr (kReduce) {
         if (fix) {
           // ---- split-K fix-up: the last K slice to arrive finishes the tile (see TcArgs::fix_out)
           __threadfence();                                                   // this thread's adds, device-wide
-          asm volatile("bar.sync 1, 128;" ::: "memory");                     // ... and those of all 128 epilogue threads
-          if (threadIdx.x == 64) *last_slot = (atomicAdd(args.fix_counters + t, 1) == (int)gridDim.z - 1) ? 1u : 0u;
-          asm volatile("bar.sync 1, 128;" ::: "memory");
+          asm volatile("bar.sync 1, 256;" ::: "memory");                     // ... and those of all 256 consumer threads
+          if (ctid == 0) *last_slot = (atomicAdd(args.fix_counters + t, 1) == (int)gridDim.z - 1) ? 1u : 0u;
+          asm volatile("bar.sync 1, 256;" ::: "memory");
           if (*(volatile uint32_t*)last_slot) {
             __threadfence();
             TcArgs fa = args;
             fa.outs[0] = args.fix_out;
             fa.ldo = args.fix_ldo;
             float* ws = static_cast<float*>(args.outs[0]);
-            if (i_glob < args.rows_a) {
+            // thread -> (tile row ctid % 128, column half ctid / 128)
+            const int fi = tc.a_row0 + (ctid & 127);
+            if (fi < args.rows_a) {
 #pragma unroll 1
-              for (int c = 0; c < BN / 16; c++) {
-                const int j0 = tc.b_row0 + c * 16;
+              for (int q = 0; q < BN / 32; q++) {
+                const int j0 = tc.b_row0 + (ctid >> 7) * (BN / 2) + q * 16;
                 if (j0 >= args.rows_b) break;
-                float acc[16];
+                float v[16];
 #pragma unroll
                 for (int u = 0; u < 16; u++) {
-                  acc[u] = 0.f;
+                  v[u] = 0.f;
                   if (j0 + u < args.rows_b) {
-                    float* p = kSwap ? ws + size_t(j0 + u) * args.ldo + i_glob : ws + size_t(i_glob) * args.ldo + j0 + u;
-                    acc[u] = __ldcg(p);
+                    float* p = kSwap ? ws + size_t(j0 + u) * args.ldo + fi : ws + size_t(fi) * args.ldo + j0 + u;
+                    v[u] = __ldcg(p);
                     __stcg(p, 0.f);                                           // the workspace is clean for the next call
                   }
                 }
-                epilogue_chunk<kSwap, false>(fa, i_glob, j0, acc, args.bias != nullptr, DeviceOut{});
+                epilogue_chunk<kSwap, false>(fa, fi, j0, v, args.bias != nullptr, DeviceOut{});
               }
             }
-            if (threadIdx.x == 64) args.fix_counters[t] = 0;
+            if (ctid == 0) args.fix_counters[t] = 0;
           }
-          asm volatile("bar.sync 1, 128;" ::: "memory");                     // last_slot is reused by the next tile
+          asm volatile("bar.sync 1, 256;" ::: "memory");                     // last_slot is reused by the next tile
         }
       }
     }
   }
-
-  // ---- teardown: every TMEM read and MMA is ordered before the barrier, then the allocating warp frees the columns
-  tc_fence_before_sync();
   __syncthreads();
-  if (warp == 1) {
-    __syncwarp();                       // lane 0 spent the kernel in the MMA loop: tcgen05.dealloc is .sync.aligned
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -458,20 +513,20 @@ int launch(const TcBatchMaps& mbatch, const CUtensorMap& mfeat, const TcArgs& a,
   return 1;
 }
 
-// SMs of the current device; 148 (B200) when there is none to ask (host-only planning in the CPU tests)
+// SMs of the current device; 132 (H100 SXM) when there is none to ask (host-only planning in the CPU tests)
 int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0, v = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0)
       n = v;
-    else { (void)cudaGetLastError(); n = 148; }
+    else { (void)cudaGetLastError(); n = 132; }
   }
   return n;
 }
 
 // `batch` / `feat`: the two operands in problem order (out[batch index, feature index]); the plan decides which of them
-// rides the TMEM lanes.  bias is indexed by the feature.  All the index logic is tc_body.cuh::setup_problem (pure, unit-
+// rides the accumulator rows.  bias is indexed by the feature.  All the index logic is tc_body.cuh::setup_problem (pure, unit-
 // tested on the CPU); here the map descriptions are encoded and the instantiation is picked.
 int run(const Operand& batch, const Operand& feat, int red, const void* bias, void* const* outs, int n_outs, int multicast,
         bool reduce, int ldo, int act, int splits, int* err_dev, void* stream, const void* const* shards = nullptr,
@@ -584,8 +639,6 @@ int run_conv_wgrad(const void* gy, const void* x, void* dw, float* ws, int* coun
 BNET_API const char* bnet_tc_last_error(void) { return g_err.c_str(); }
 BNET_API uint64_t bnet_tc_smem_desc(uint32_t smem_addr) { return smem_desc_sw128(smem_addr); }
 BNET_API uint64_t bnet_tc_smem_desc_mn(uint32_t smem_addr) { return smem_desc_sw128_mn(smem_addr); }
-BNET_API uint32_t bnet_tc_instr_desc(int m, int n) { return instr_desc_bf16_f32(m, n); }
-BNET_API uint32_t bnet_tc_instr_desc2(int m, int n, int a_mn, int b_mn) { return instr_desc_bf16_f32(m, n, a_mn != 0, b_mn != 0); }
 
 BNET_API int bnet_tc_supported(void) {
   int dev = 0, major = 0;
@@ -593,7 +646,7 @@ BNET_API int bnet_tc_supported(void) {
     (void)cudaGetLastError();
     return 0;
   }
-  return (major == 10 && encode_fn() != nullptr) ? 1 : 0;
+  return (major == 9 && encode_fn() != nullptr) ? 1 : 0;
 }
 
 BNET_API int bnet_tc_plan(int M, int N, int K, int reduce, int splits, BnetTcPlan* p) {
@@ -616,7 +669,7 @@ BNET_API int bnet_tc_linear_reduce(const void* x, const void* w, const void* bia
 }
 
 // Split-K with the finish inside the kernel: `ws` is an fp32 [M, N] workspace and `counters` one int per output tile
-// (bnet_tc_plan: grid_x * grid_y), BOTH all zero on entry — the kernel leaves them all zero again, so they are allocated
+// (bnet_tc_plan: grid_x * grid_y) plus one, BOTH all zero on entry — the kernel leaves them all zero again, so they are allocated
 // and cleared once.  out = act(x . w^T + bias) in bf16, one launch.
 BNET_API int bnet_tc_linear_splitk(const void* x, const void* w, const void* bias, void* out, float* ws, int* counters, int M, int N,
                                    int K, int ldx, int ldw, int ldo, int act, int splits, int* err_dev, void* stream) {

@@ -58,7 +58,7 @@ ncclResult_t fill_common(int dev, DeviceProps* p, char** name, char** pci) {
 // NCCL drives a net plugin through a proxy pipeline of NCCL_BUFFSIZE/8-byte slices per channel, and for small and
 // medium messages it prefers the LL protocol, whose buffers live in host memory (so they ride our shared-memory
 // ring, not NVLink).  Over this transport the measured optimum is the Simple protocol with large slices and many
-// channels (profiles/README.md section 4).  NCCL reads these variables after the plugin's init(), so a default can
+// channels.  NCCL reads these variables after the plugin's init(), so a default can
 // be supplied here; anything the user has set wins, BNET_TUNE_NCCL=0 leaves the environment alone.
 void tune_nccl_env() {
   if (env_int("TUNE_NCCL", 1) == 0) return;

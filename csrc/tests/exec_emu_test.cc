@@ -1,8 +1,8 @@
 // CPU emulation test of the transport executor's data-movement bodies (csrc/cuda/exec_body.cuh): the same
-// process_range()/cta_share() the sm_100a kernels inline, compiled by g++ and run as an emulated cluster
+// process_range()/cta_share() the sm_90a kernels inline, compiled by g++ and run as an emulated cluster
 // (every CTA, every thread, serially) over every op, odd sizes and unaligned offsets, against scalar references.
 // Serial emulation is exact here: each destination element is touched by exactly one thread.
-// (tests/test_gpu.py::test_executor_copy_reduce_cast runs the real kernels against PyTorch on a B200.)
+// (tests/test_gpu.py::test_executor_copy_reduce_cast runs the real kernels against PyTorch on an H100.)
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -2,7 +2,7 @@
 // csrc/cuda/nn_body.cuh with g++ and walks an emulated grid (every block, every thread, serially), then
 // compares with a straightforward scalar reference.  Checks the strided row walk, the tail handling of the
 // unrolled load batches, the pool index coding and that every output element is written exactly as expected.
-// (The same kernels are compared against PyTorch on a real B200 by tests/test_gpu.py::test_fused_nn.)
+// (The same kernels are compared against PyTorch on a real H100 by tests/test_gpu.py::test_fused_nn.)
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

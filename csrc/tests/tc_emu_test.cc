@@ -1,10 +1,11 @@
-// The tcgen05 linear kernel's index logic (csrc/cuda/tc_body.cuh) on an emulated TMA / MMA / TMEM, no GPU needed.
+// The wgmma linear kernel's index logic (csrc/cuda/tc_body.cuh) on an emulated TMA / MMA / accumulator, no GPU needed.
 //
 // What runs here is the code the kernel runs: setup_problem (orientation, tensor-map descriptions, kernel arguments),
 // tile_coord (tile -> rows, gathered shard), stage_loads (which TMA boxes, at which coordinates, where in the stage) and
 // epilogue_chunk (bias / ReLU / bf16 store, cross-rank adds, reduce-scatter).  What is emulated: the TMA engine (a box
 // copy with zero fill), the MMA (a dot product over the stage as the shared-memory descriptors describe it: K-major
-// rows, or MN-major 64 x 64 atoms 8 KiB apart) and TMEM (a float array).  Every mode is compared with a plain GEMM.
+// rows, or MN-major 64 x 64 atoms 8 KiB apart) and the register accumulator (a float array).  Every mode is compared with a
+// plain GEMM.
 //
 //   make build/tests/tc_emu_test && build/tests/tc_emu_test
 #include <math.h>
@@ -65,7 +66,7 @@ static void run_kernel(const Problem& pr, const HostOut& out) {
   const TcArgs& args = pr.args;
   const BnetTcPlan& p = pr.plan;
   std::vector<uint16_t> stage_a(kABytes / 2), stage_b(BN * kBK);
-  std::vector<float> tmem(size_t(kBM) * BN);
+  std::vector<float> accum(size_t(kBM) * BN);
   for (int z = 0; z < p.grid_z; z++) {
     const int kb_begin = z * args.k_per_split;
     const int kb_end = kb_begin + args.k_per_split < args.k_blocks ? kb_begin + args.k_per_split : args.k_blocks;
@@ -73,7 +74,7 @@ static void run_kernel(const Problem& pr, const HostOut& out) {
     for (int cta = 0; cta < p.ctas; cta++) {
       for (int t = cta; t < args.n_tiles; t += p.ctas) {
         const TileCoord tc = tile_coord<BN, kSwap>(args, t);
-        std::fill(tmem.begin(), tmem.end(), 0.f);
+        std::fill(accum.begin(), accum.end(), 0.f);
         for (int kb = kb_begin; kb < kb_end; kb++) {
           std::fill(stage_a.begin(), stage_a.end(), uint16_t(0x7fc0));     // stale data must never be read
           std::fill(stage_b.begin(), stage_b.end(), uint16_t(0x7fc0));
@@ -89,17 +90,20 @@ static void run_kernel(const Problem& pr, const HostOut& out) {
             for (int j = 0; j < BN; j++) {
               float s = 0.f;
               for (int k = 0; k < kBK; k++) s += stage_at(stage_a.data(), kAMn, i, k) * stage_at(stage_b.data(), kBMn, j, k);
-              tmem[size_t(i) * BN + j] += s;
+              accum[size_t(i) * BN + j] += s;
             }
         }
         const bool add_bias = args.bias != nullptr && (!kReduce || z == 0);
-        for (int warp = 2; warp < 6; warp++)
+        // the kernel's consumer warps 4 .. 11: warp w takes rows 64 (w / 4 - 1) + 16 (w % 4) .. +15, and per 32-column chunk
+        // lane l finishes row l % 16, columns 16 (l / 16) .. +15
+        for (int warp = 4; warp < 12; warp++)
           for (int lane = 0; lane < 32; lane++) {
-            const int q = warp & 3, i_local = q * 32 + lane;
-            for (int c = 0; c < BN / 16; c++) {
+            const int i_local = 64 * (warp / 4 - 1) + 16 * (warp % 4) + (lane & 15);
+            for (int cc = 0; cc < BN / 32; cc++) {
+              const int col = 32 * cc + 16 * (lane >> 4);
               float acc[16];
-              for (int u = 0; u < 16; u++) acc[u] = tmem[size_t(i_local) * BN + c * 16 + u];
-              epilogue_chunk<kSwap, kReduce>(args, tc.a_row0 + i_local, tc.b_row0 + c * 16, acc, add_bias, out);
+              for (int u = 0; u < 16; u++) acc[u] = accum[size_t(i_local) * BN + col + u];
+              epilogue_chunk<kSwap, kReduce>(args, tc.a_row0 + i_local, tc.b_row0 + col, acc, add_bias, out);
             }
           }
       }
@@ -169,7 +173,7 @@ static void reduce(int M, int N, int K, int n_outs, bool multicast, int splits, 
   int err = 0;
   Problem pr;
   const char* e = setup_problem(Operand{x.ptr(), M, x.ld, 0}, Operand{w.ptr(), N, w.ld, 0}, K, bias ? b.ptr() : nullptr, outs, n,
-                                multicast ? 1 : 0, true, N, 0, splits, &err, nullptr, 0, scatter, 148, &pr);
+                                multicast ? 1 : 0, true, N, 0, splits, &err, nullptr, 0, scatter, 132, &pr);
   CHECK(e == nullptr, "setup: %s", e ? e : "");
   if (e) return;
   CHECK(dispatch(pr, true, ho), "no kernel for reduce %dx%dx%d", M, N, K);
@@ -227,7 +231,7 @@ static void backward(int M, int N, int K) {
   Problem pr;
   void* o1[1] = {dx};
   const char* e = setup_problem(Operand{gy.ptr(), M, gy.ld, 0}, Operand{w.ptr(), K, w.ld, 1}, N, nullptr, o1, 1, 0, false, K, 0, 1, &err,
-                                nullptr, 0, 0, 148, &pr);
+                                nullptr, 0, 0, 132, &pr);
   CHECK(e == nullptr, "dgrad setup: %s", e ? e : "");
   if (!e) {
     CHECK(dispatch(pr, false, HostOut{}), "no kernel for dgrad %dx%dx%d (swap %d bn %d)", M, N, K, pr.plan.swap, pr.plan.bn);
@@ -243,7 +247,7 @@ static void backward(int M, int N, int K) {
   if (N <= 64) return;
   void* o2[1] = {dw};
   e = setup_problem(Operand{gy.ptr(), N, gy.ld, 1}, Operand{x.ptr(), K, x.ld, 1}, M, nullptr, o2, 1, 0, false, K, 0, 1, &err, nullptr, 0, 0,
-                    148, &pr);
+                    132, &pr);
   CHECK(e == nullptr, "wgrad setup: %s", e ? e : "");
   if (e) return;
   CHECK(dispatch(pr, false, HostOut{}), "no kernel for wgrad %dx%dx%d", M, N, K);
@@ -257,7 +261,7 @@ static void backward(int M, int N, int K) {
   CHECK(bad == 0, "wgrad M=%d N=%d K=%d: %d wrong", M, N, K, bad);
 }
 
-// ---- convolution (implicit GEMM): 4-D boxes with zero fill, the same MMA / TMEM emulation -------------------------------
+// ---- convolution (implicit GEMM): 4-D boxes with zero fill, the same MMA / accumulator emulation ------------------------
 static void tma_box4(const MapDesc4& d, int c0, int c1, int c2, int c3, uint16_t* dst) {
   const uint16_t* src = static_cast<const uint16_t*>(d.ptr);
   size_t o = 0;
@@ -276,12 +280,12 @@ static void run_conv_kernel(const ConvProblem& cp, const HostOut& out) {
   const TcArgs& args = cp.args;
   const BnetTcPlan& p = cp.plan;
   std::vector<uint16_t> stage_a(kABytes / 2), stage_b(BN * kBK);
-  std::vector<float> tmem(size_t(kBM) * BN);
+  std::vector<float> accum(size_t(kBM) * BN);
   CHECK(args.conv.bw * args.conv.bh * args.conv.bn == kBM, "patch %d x %d x %d", args.conv.bw, args.conv.bh, args.conv.bn);
   for (int cta = 0; cta < p.ctas; cta++)
     for (int t = cta; t < args.n_tiles; t += p.ctas) {
       const ConvTile ct = conv_tile<BN>(args, t);
-      std::fill(tmem.begin(), tmem.end(), 0.f);
+      std::fill(accum.begin(), accum.end(), 0.f);
       for (int kb = 0; kb < args.k_blocks; kb++) {
         std::fill(stage_a.begin(), stage_a.end(), uint16_t(0x7fc0));
         std::fill(stage_b.begin(), stage_b.end(), uint16_t(0x7fc0));
@@ -294,7 +298,7 @@ static void run_conv_kernel(const ConvProblem& cp, const HostOut& out) {
           for (int j = 0; j < BN; j++) {
             float s = 0.f;
             for (int k = 0; k < kBK; k++) s += stage_at(stage_a.data(), false, i, k) * stage_at(stage_b.data(), kBMn, j, k);
-            tmem[size_t(i) * BN + j] += s;
+            accum[size_t(i) * BN + j] += s;
           }
       }
       for (int r = 0; r < kBM; r++) {
@@ -302,7 +306,7 @@ static void run_conv_kernel(const ConvProblem& cp, const HostOut& out) {
         const int i_glob = row < 0 ? args.rows_a : (int)row;
         for (int c = 0; c < BN / 16; c++) {
           float acc[16];
-          for (int u = 0; u < 16; u++) acc[u] = tmem[size_t(r) * BN + c * 16 + u];
+          for (int u = 0; u < 16; u++) acc[u] = accum[size_t(r) * BN + c * 16 + u];
           epilogue_chunk<false, false>(args, i_glob, ct.b_row0 + c * 16, acc, args.bias != nullptr, out);
         }
       }
@@ -375,7 +379,7 @@ static void run_wgrad_kernel(const WgradProblem& wp, const HostOut& out) {
   const TcArgs& args = wp.args;
   const BnetTcPlan& p = wp.plan;
   std::vector<uint16_t> stage_a(kABytes / 2), stage_b(BN * kBK);
-  std::vector<float> tmem(size_t(kBM) * BN);
+  std::vector<float> accum(size_t(kBM) * BN);
   CHECK(args.conv.bw * args.conv.bh * args.conv.bn == 64, "wgrad patch %d x %d x %d", args.conv.bw, args.conv.bh, args.conv.bn);
   CHECK(wp.gy_map.bw * wp.gy_map.bh * wp.gy_map.bn == 64 && wp.x_map.bw * wp.x_map.bh * wp.x_map.bn == 64, "wgrad boxes");
   int* counters = args.fix_counters;
@@ -387,7 +391,7 @@ static void run_wgrad_kernel(const WgradProblem& wp, const HostOut& out) {
     for (int cta = 0; cta < p.ctas; cta++)
       for (int t = cta; t < args.n_tiles; t += p.ctas) {
         const TileCoord tc = tile_coord<BN, false>(args, t);
-        std::fill(tmem.begin(), tmem.end(), 0.f);
+        std::fill(accum.begin(), accum.end(), 0.f);
         for (int kb = kb_begin; kb < kb_end; kb++) {
           std::fill(stage_a.begin(), stage_a.end(), uint16_t(0x7fc0));
           std::fill(stage_b.begin(), stage_b.end(), uint16_t(0x7fc0));
@@ -400,14 +404,14 @@ static void run_wgrad_kernel(const WgradProblem& wp, const HostOut& out) {
             for (int j = 0; j < BN; j++) {
               float s = 0.f;
               for (int k = 0; k < kBK; k++) s += stage_at(stage_a.data(), true, i, k) * stage_at(stage_b.data(), true, j, k);
-              tmem[size_t(i) * BN + j] += s;
+              accum[size_t(i) * BN + j] += s;
             }
         }
         // the epilogue of the reduce instantiation: fp32 adds into the workspace ...
         for (int r = 0; r < kBM; r++)
           for (int c = 0; c < BN / 16; c++) {
             float acc[16];
-            for (int u = 0; u < 16; u++) acc[u] = tmem[size_t(r) * BN + c * 16 + u];
+            for (int u = 0; u < 16; u++) acc[u] = accum[size_t(r) * BN + c * 16 + u];
             epilogue_chunk<false, true>(args, tc.a_row0 + r, tc.b_row0 + c * 16, acc, false, out);
           }
         // ... and the fix-up: the slice that arrives last at the tile reads the sums back, writes bf16, re-zeroes what it read
@@ -489,28 +493,28 @@ static void conv_wgrad(int N, int H, int W, int Cin, int Cout, int sms, int spli
 int main() {
   // filter gradients: exact and ragged 64-pixel patches, Cout below / above one lane tile, tiles that straddle taps (Cin = 64
   // with 128 columns), columns past 9 * Cin (Cin = 128 with 256-column tiles), one slice / many slices / persistent CTAs
-  conv_wgrad(2, 8, 8, 64, 64, 148, 0);
+  conv_wgrad(2, 8, 8, 64, 64, 132, 0);
   conv_wgrad(3, 7, 7, 64, 128, 4, 0);
-  conv_wgrad(1, 14, 14, 128, 64, 148, 3);
+  conv_wgrad(1, 14, 14, 128, 64, 132, 3);
   conv_wgrad(5, 4, 4, 64, 192, 2, 1);
   conv_wgrad(2, 6, 10, 128, 256, 7, 0);
-  conv_wgrad(1, 5, 3, 256, 128, 148, 0);
+  conv_wgrad(1, 5, 3, 256, 128, 132, 0);
   conv_wgrad(2, 6, 10, 128, 256, 7, 0, 128);         // the self-check's fallback: 128-column tiles for every layer
-  conv_wgrad(1, 5, 3, 256, 128, 148, 2, 128);
+  conv_wgrad(1, 5, 3, 256, 128, 132, 2, 128);
   conv_wgrad(3, 7, 7, 64, 128, 4, 0, 0, 0);          // ... and without the in-kernel finish (the caller converts the workspace)
   conv_wgrad(2, 6, 10, 128, 256, 7, 2, 128, 0);
   // forward / input gradient: exact patches, ragged patches (7x7, 14x14 with odd batch), several images per patch, persistent CTAs
-  conv(2, 8, 16, 64, 64, true, 148);
+  conv(2, 8, 16, 64, 64, true, 132);
   conv(3, 7, 7, 64, 128, false, 3);
   conv(1, 14, 14, 128, 64, true, 2);
-  conv(5, 4, 4, 64, 72, true, 148);
+  conv(5, 4, 4, 64, 72, true, 132);
   conv(2, 10, 6, 64, 320, false, 1);
   // forward: both orientations, ragged extents, row pitches, one tile per CTA and persistent (few "SMs")
-  forward(32, 256, 512, true, true, 148, 0);
-  forward(48, 200, 264, true, false, 148, 16);
-  forward(1, 8, 8, false, false, 148, 0);
+  forward(32, 256, 512, true, true, 132, 0);
+  forward(48, 200, 264, true, false, 132, 16);
+  forward(1, 8, 8, false, false, 132, 0);
   forward(64, 130, 72, true, true, 2, 0);
-  forward(130, 136, 72, true, false, 148, 8);
+  forward(130, 136, 72, true, false, 132, 8);
   forward(257, 129, 200, false, true, 3, 0);
   forward(300, 520, 136, true, true, 4, 0);
   forward(256, 512, 64, true, false, 2, 0);           // 128 x 256 tiles (2 x 2 of them >= 2 SMs)

@@ -11,7 +11,7 @@
 //   receiver irecv : rdesc[k%S] = {capacity, mr, offset, type}; seq=k+1 (release)
 //   sender   isend : waits for rdesc seq, then announces ann[k%S] = {nbytes, path}
 //     direct path  : dst is a registered CUDA buffer we could import ->
-//                    sm_100a copy kernel writes the peer buffer over NVLink, one
+//                    sm_90a copy kernel writes the peer buffer over NVLink, one
 //                    completion word per chunk; host then publishes done[k%S]
 //     ring path    : payload streams through an SPSC byte ring in the shm
 //                    (host<->host, or CUDA staged with private-stream copies)
@@ -486,7 +486,7 @@ class NvlComm : public Comm {
     if (!(gen & 1)) return nullptr;
     Import& im = imports_[mr_idx];
     if (im.gen != gen) {
-      // unmapping waits for running kernels (profiles/blocking_calls.txt): never on the data path
+      // unmapping waits for running kernels (tools/blocking_calls_probe.py): never on the data path
       if (im.base) stale_.push_back(im);
       im = Import();
       im.gen = gen;

@@ -17,7 +17,7 @@ def main():
     comm = SymmComm(256 << 20)
     if not (tc_linear.enabled() and tc_linear.self_check(verbose=comm.rank == 0)):
         if comm.rank == 0:
-            print("tcgen05 path disabled (BNET_TC=0), unsupported on this GPU, or its self-check failed")
+            print("wgmma path disabled (BNET_TC=0), unsupported on this GPU, or its self-check failed")
         return
     M, N, K = 512, 4096, 8192
     torch.manual_seed(0)

@@ -3,7 +3,7 @@
  *
  * The reference moves bytes for NCCL and leaves the reduction to NCCL's kernels
  * (SURVEY.md §2.5, K4-K6 in §2.6).  On an NVSwitch box the transport and the
- * reduction fuse: these entry points run hand-written sm_100a kernels that reduce
+ * reduction fuse: these entry points run hand-written sm_90a kernels that reduce
  * in the switch (NVLS multimem.ld_reduce / multimem.st on a cuMulticast mapping) or
  * with peer loads/stores over NVLink, optionally fused with the optimizer step.
  *

@@ -1,5 +1,5 @@
 /*
- * bnet tensor-core linear — tcgen05 / TMEM / TMA GEMM with a fused epilogue, optionally fused with the all-reduce
+ * bnet tensor-core linear — wgmma / TMA GEMM with a fused epilogue, optionally fused with the all-reduce
  * of a row-parallel (tensor-parallel) linear layer.
  *
  *   out[M,N] = act(x[M,K] . w[N,K]^T + bias[N])                       bnet_tc_linear        (bf16 in, bf16 out)
@@ -10,11 +10,11 @@
  * vector through the NVSwitch multicast mapping, or one red.global per peer over NVLink — so the transfer of tile t
  * overlaps the math of tile t+1.  The caller zeroes the output, runs a rank barrier before and after (bnet_barrier).
  *
- * The reference has no counterpart (it moves bytes for NCCL; SURVEY.md §2.6): this is the B200 "compute step followed
- * by a collective" path.  STATUS: validated on B200 in round 2 (profiles/r2/tc_probe_1gpu.txt; on by default, BNET_TC=0
- * disables); descriptor packing is checked against the CuTe definitions on the host (tests/test_utils.py), and every
- * launch carries a watchdog that turns a stuck pipeline into an error code instead of a hang.  The convolution filter
- * gradient (bnet_tc_conv3x3_wgrad) came after the last hardware session: CPU-emulated only, see ops/tc_conv.py.
+ * The reference has no counterpart (it moves bytes for NCCL; SURVEY.md §2.6): this is the GPU "compute step followed
+ * by a collective" path (on by default, BNET_TC=0 disables); descriptor packing is checked against the CuTe definitions on
+ * the host (tests/test_utils.py), and every launch carries a watchdog that turns a stuck pipeline into an error code
+ * instead of a hang.  Callers in Python trust the kernels only after a self-check on the GPU at hand (ops/tc_linear.py,
+ * ops/tc_conv.py).
  */
 #ifndef BNET_TC_H_
 #define BNET_TC_H_
@@ -29,12 +29,12 @@ enum { BNET_TC_ACT_NONE = 0, BNET_TC_ACT_RELU = 1 };
 #define BNET_TC_MAX_OUTS 16
 #define BNET_TC_MAX_PEERS 8
 
-/* 1 when the driver exposes cuTensorMapEncodeTiled and the current device is compute capability 10.x */
+/* 1 when the driver exposes cuTensorMapEncodeTiled and the current device is compute capability 9.x (sm_90a) */
 int bnet_tc_supported(void);
 
 /* How a problem is tiled (pure host function; also used by the tests).  Returns 0 and fills the plan, or -1. */
 typedef struct BnetTcPlan {
-  int swap;       /* 1: w rows fill the 128 TMEM lanes and x rows are the MMA N dimension (small batch) */
+  int swap;       /* 1: w rows fill the 128 accumulator rows and x rows are the MMA N dimension (small batch) */
   int bn;         /* MMA N (tile width of the other operand): 32 / 64 (swapped), 128 or 256 */
   int stages;     /* TMA -> MMA shared-memory pipeline depth */
   int grid_x, grid_y, grid_z;   /* tiles along the column operand, tiles along the lane operand, K slices */
@@ -51,7 +51,7 @@ int bnet_tc_linear(const void* x, const void* w, const void* bias, void* out, in
 
 /* Split-K for weight-streaming (small batch) layers with the finish fused into the kernel: K is cut into `splits` slices
  * so that every SM streams weights; partial tiles meet as fp32 adds in `ws` ([M, N] floats), and the slice that arrives
- * last at a tile (counted in `counters`, one int per output tile) applies bias / activation and writes the bf16 result.
+ * last at a tile (counted in `counters`, one int per output tile plus one) applies bias / activation and writes the bf16 result.
  * `ws` and `counters` must be all zero on entry and are all zero again on exit.  One launch. */
 int bnet_tc_linear_splitk(const void* x, const void* w, const void* bias, void* out, float* ws, int* counters, int M, int N, int K,
                           int ldx, int ldw, int ldo, int act, int splits, int* err_dev, void* stream);
@@ -82,7 +82,7 @@ int bnet_tc_linear_wgrad(const void* gy, const void* x, void* dw, int M, int N, 
 
 /* 3x3 / stride 1 / pad 1 convolution as an implicit GEMM on the same kernel: the 128 accumulator rows of a tile are a
  * patch of output pixels whose (shifted) inputs arrive as 4-D TMA boxes of the NHWC activation — padding = the TMA unit's
- * zero fill — and bias + ReLU are applied from TMEM.  bf16 NHWC activations, filters [Cout][3][3][Cin] (the memory of a
+ * zero fill — and bias + ReLU are applied in the epilogue.  bf16 NHWC activations, filters [Cout][3][3][Cin] (the memory of a
  * channels_last torch Conv2d weight).  Cin % 64 == 0, Cout % 8 == 0.  dgrad reads the SAME filter MN-major with flipped
  * taps (Cin % 64 == 0 and Cout % 64 == 0). */
 int bnet_tc_conv3x3(const void* x, const void* w, const void* bias, void* out, int N, int H, int W, int Cin, int Cout, int act,
@@ -99,12 +99,10 @@ int bnet_tc_conv3x3_wgrad(const void* gy, const void* x, void* dw, float* ws, in
 int bnet_tc_conv3x3_wgrad_tiles(int Cin, int Cout);
 int bnet_tc_conv3x3_wgrad_plan(int N, int H, int W, int Cin, int Cout, int splits, BnetTcPlan* plan);   /* host only */
 
-/* The 64-bit shared-memory matrix descriptor (K-major, 128-byte swizzle) and the 32-bit instruction descriptor
- * (bf16 x bf16 -> fp32) the kernel issues, exposed so a host test can compare them with the CuTe definitions. */
+/* The 64-bit wgmma shared-memory matrix descriptor (K-major, 128-byte swizzle) the kernel issues, exposed so a host test
+ * can compare it with the CuTe definition. */
 uint64_t bnet_tc_smem_desc(uint32_t smem_addr);
 uint64_t bnet_tc_smem_desc_mn(uint32_t smem_addr);            /* MN-major tile staged as 64 x 64 boxes */
-uint32_t bnet_tc_instr_desc(int m, int n);
-uint32_t bnet_tc_instr_desc2(int m, int n, int a_mn_major, int b_mn_major);
 
 const char* bnet_tc_last_error(void);
 

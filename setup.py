@@ -1,4 +1,4 @@
-"""`pip install --no-build-isolation .` — runs `make` (g++ + nvcc for sm_100a; no GPU needed) and ships the three plugin
+"""`pip install --no-build-isolation .` — runs `make` (g++ + nvcc for sm_90a; no GPU needed) and ships the three plugin
 variants inside the package (bagua_net_b200/lib/).  Working from a checkout needs none of this: the library is built in
 the tree on first use (bagua_net_b200._build) and `make install PREFIX=...` copies the plugin for NCCL alone.
 Counterpart of the reference's `make && make install` (reference: cc/Makefile, README.md:32-45)."""

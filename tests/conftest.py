@@ -1,7 +1,7 @@
 """pytest config: registers the `gpu` marker and makes sure the native library exists.
 
 CPU tests (`-m "not gpu"`) exercise the host engine, the TCP/shared-memory transports
-and the plugin ABI over loopback; GPU tests (`-m gpu`) need a real B200.
+and the plugin ABI over loopback; GPU tests (`-m gpu`) need a real H100.
 """
 import os
 import subprocess
@@ -15,7 +15,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a B200 with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
 
 

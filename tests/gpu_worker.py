@@ -595,12 +595,12 @@ def job_fused_bn():
 
 
 def job_tc_linear():
-    """tcgen05 linear (csrc/cuda/tc_gemm.cu) vs an fp32 PyTorch reference: both operand orientations, ragged M/N/K,
+    """wgmma linear (csrc/cuda/tc_gemm.cu) vs an fp32 PyTorch reference: both operand orientations, ragged M/N/K,
     bias, ReLU, non-trivial row pitches, and the autograd wrapper."""
     from bagua_net_b200.ops import tc_linear
 
     setup()
-    assert tc_linear.supported(), "tcgen05 linear reports unsupported on this GPU / driver"
+    assert tc_linear.supported(), "wgmma linear reports unsupported on this GPU / driver"
     assert tc_linear.self_check(verbose=True), "tc_linear self-check failed"
     torch.manual_seed(3)
     for (M, N, K) in [(1, 8, 8), (32, 4096, 25088), (64, 1000, 4096), (65, 520, 200), (512, 512, 4096), (1000, 1000, 1000)]:
@@ -1052,26 +1052,26 @@ def job_tc_conv():
 
     setup()
     assert tc_linear.supported()
-    assert tc_conv.self_check(verbose=RANK == 0), "tcgen05 convolution differs from cuDNN"
-    print("tcgen05 conv3x3 forward + dgrad match cuDNN", flush=True)
+    assert tc_conv.self_check(verbose=RANK == 0), "wgmma convolution differs from cuDNN"
+    print("wgmma conv3x3 forward + dgrad match cuDNN", flush=True)
     teardown()
 
 
 def job_tc_conv_wgrad():
-    """The tcgen05 filter gradient against cuDNN (several shapes, one and many pixel slices, scratch handed back clean),
+    """The wgmma filter gradient against cuDNN (several shapes, one and many pixel slices, scratch handed back clean),
     then inside a fused conv block: the autotuner may pick it per shape, training must look the same either way."""
     from bagua_net_b200.ops import tc_conv, tc_linear
 
     setup()
     assert tc_linear.supported()
-    assert tc_conv.self_check_wgrad(verbose=RANK == 0), "tcgen05 filter gradient differs from cuDNN"
+    assert tc_conv.self_check_wgrad(verbose=RANK == 0), "wgmma filter gradient differs from cuDNN"
     os.environ["BNET_TC_WGRAD"] = "1"          # just checked in this very process
     x = torch.randn(8, 128, 28, 28, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last)
     gy = torch.randn(8, 256, 28, 28, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last) / 28
     w = torch.randn(256, 128, 3, 3, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last)
     ref = lambda: torch.ops.aten.convolution_backward(gy, x, w, None, [1, 1], [1, 1], [1, 1], False, [0, 0], 1, [False, True, False])[1]   # noqa: E731
     pick = tc_conv.choose_wgrad(gy, x, w, ref)
-    print(f"tcgen05 conv3x3 filter gradient matches cuDNN; autotuner for 128->256 @28: {pick} {tc_conv.TIMINGS}", flush=True)
+    print(f"wgmma conv3x3 filter gradient matches cuDNN; autotuner for 128->256 @28: {pick} {tc_conv.TIMINGS}", flush=True)
     teardown()
 
 

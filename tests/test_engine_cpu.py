@@ -125,7 +125,7 @@ def test_engine_trains_like_torch_sgd(cpu_engine, channels_last):
 
 
 class _LinearDirect(torch.autograd.Function):
-    """A linear layer whose backward uses ops.tc_linear.weight_grad (its library path: torch.mm with out=): what the tcgen05
+    """A linear layer whose backward uses ops.tc_linear.weight_grad (its library path: torch.mm with out=): what the wgmma
     classifier does on a GPU, minus the kernel."""
 
     @staticmethod

@@ -1,4 +1,4 @@
-"""GPU tests (run on a B200 with `pytest -m gpu`).  Every kernel is compared against a plain
+"""GPU tests (run on an H100 with `pytest -m gpu`).  Every kernel is compared against a plain
 PyTorch fp32 reference of the same op.  Multi-GPU cases launch one process per GPU and are
 skipped on a single-GPU box."""
 import json
@@ -189,9 +189,8 @@ def test_executor_single_grid_mode(env):
     _run_worker("executor_idle", 1, extra_env=dict(env, BNET_KERNEL_IDLE_US="100"), timeout=60)
 
 
-# ------------------------------------------------------------------ tcgen05 linear / convolution / fused GEMM + all-reduce
-# (validated on B200 in round 2: profiles/r2/tc_probe_1gpu.txt; the kernel's waits carry a watchdog, so a wrong pipeline
-#  fails instead of hanging)
+# ------------------------------------------------------------------ wgmma linear / convolution / fused GEMM + all-reduce
+# (the kernel's waits carry a watchdog, so a wrong pipeline fails instead of hanging)
 def test_tcgen05_linear_matches_fp32_reference():
     _run_worker("tc_linear", 1, timeout=240)
 
@@ -282,14 +281,14 @@ def test_nccl_collnet_probe_2gpu():
     print("collnet all-reduces executed by the plugin (min over ranks):", d["collnet_allreduces_min_over_ranks"])
 
 
-# ------------------------------------------------------------------ written after the last hardware session of round 2: LAST in the file
+# ------------------------------------------------------------------ the newest paths: LAST in the file
 def test_executor_fp8_decompression_ops():
     """fp8 -> fp32 overwrite ops (OP_CAST_E4M3_TO_F32 / OP_CAST_E5M2_TO_F32) of the compressed all-reduce's all-gather half."""
     _run_worker("executor_decompress", 1, timeout=120)
 
 
 def test_tcgen05_conv3x3_filter_gradient_matches_cudnn():
-    """tcgen05 weight gradient (both operands 64-pixel 4-D TMA boxes, MN-major; split over the pixels with the fix-up)."""
+    """wgmma weight gradient (both operands 64-pixel 4-D TMA boxes, MN-major; split over the pixels with the fix-up)."""
     _run_worker("tc_conv_wgrad", 1, timeout=300)
 
 

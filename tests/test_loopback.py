@@ -409,7 +409,7 @@ def test_per_gpu_virtual_devices():
     props = json.loads(out.stdout.splitlines()[-1])
     assert len(props) >= 2
     g = props[0]
-    assert g["name"] == "bnet-gpu0" and g["ptrSupport"] == 3 and g["speed"] == 7200000 and g["maxRecvs"] == 1
+    assert g["name"] == "bnet-gpu0" and g["ptrSupport"] == 3 and g["speed"] == 3600000 and g["maxRecvs"] == 1
     assert not g["pciPath"]        # a virtual NVLink "NIC" has no PCI leaf of its own (never the GPU's: see engine.cc)
     assert all(not p["name"].startswith("bnet-gpu") for p in props[1:])           # the NIC devices follow
     assert len({p["guid"] for p in props}) == len(props)

@@ -1,13 +1,13 @@
-"""A small executable model of the tcgen05 linear kernel's synchronisation (csrc/cuda/tc_gemm.cu): the three roles
-(TMA producer, MMA issuer, epilogue), the shared-memory ring that runs through tile boundaries, the double-buffered
-TMEM accumulator, and the exact parity expressions the kernel passes to its mbarrier waits.  mbarriers are modelled with
-their phase semantics (``try_wait.parity(P)`` succeeds once the phase of parity P has completed).  A random scheduler
-interleaves the roles; the model asserts what the hardware would silently get wrong:
+"""A small executable model of the wgmma linear kernel's synchronisation (csrc/cuda/tc_gemm.cu): the TMA producer and the
+two consumer warpgroups, the shared-memory ring that runs through tile boundaries, the asynchronous MMA groups (a stage
+is released only once the group that reads it has completed: one group stays in flight), and the exact parity
+expressions the kernel passes to its mbarrier waits.  mbarriers are modelled with their phase semantics
+(``try_wait.parity(P)`` succeeds once the phase of parity P has completed).  A random scheduler interleaves the roles;
+the model asserts what the hardware would silently get wrong:
 
-* a ring stage is never refilled before the MMAs that read it were committed,
+* a ring stage is never refilled before both warpgroups released it, nor while an MMA group still reads it,
 * an MMA never reads a stage that has not been filled for this k-block,
-* an accumulator stage is never overwritten before the epilogue drained it, and never read before it is complete,
-* nobody dead-locks, and every tile comes out with the right (tile, k-block) contributions.
+* nobody dead-locks, and every tile comes out of both warpgroups with the right (tile, k-block) contributions.
 
 The kernel itself cannot run here (no GPU); this guards the protocol when the loops are edited."""
 import random
@@ -29,15 +29,14 @@ class MBar:
         return self.phase != parity
 
 
-def run_model(n_tiles, grid, cta, nkb, stages, seed, epi_threads=4, bug=None):
+def run_model(n_tiles, grid, cta, nkb, stages, seed, consumers=2, bug=None):
     """One CTA of the persistent kernel.  Roles are generators that yield while blocked or between steps."""
     rng = random.Random(seed)
     full = [MBar(1) for _ in range(stages)]
-    empty = [MBar(1) for _ in range(stages)]
-    acc_full = [MBar(1) for _ in range(2)]
-    acc_empty = [MBar(epi_threads) for _ in range(2)]
-    ring = [None] * stages              # (tile, kblock) currently in the stage, None = consumed / never filled
-    acc = [None, None]                  # per accumulator stage: {"tile": t, "ks": [...], "complete": bool} or None
+    empty = [MBar(consumers) for _ in range(stages)]
+    ring = [None] * stages              # (tile, kblock) currently in the stage
+    need = [set() for _ in range(stages)]       # warpgroups that have not released the stage yet
+    reading = [set() for _ in range(stages)]    # warpgroups whose issued MMA group on the stage has not completed
     results = {}
     my_tiles = list(range(cta, n_tiles, grid))
 
@@ -49,72 +48,64 @@ def run_model(n_tiles, grid, cta, nkb, stages, seed, epi_threads=4, bug=None):
                 if rnd > 0 and bug != "producer_never_waits":
                     while not empty[s].passed((rnd & 1) if bug == "producer_parity" else ((rnd - 1) & 1)):
                         yield
-                assert ring[s] is None, f"stage {s} refilled while ({ring[s]}) is unread"
+                assert not need[s], f"stage {s} refilled while ({ring[s]}) is unread by {need[s]}"
+                assert not reading[s], f"stage {s} refilled while an MMA group of {reading[s]} still reads it"
                 ring[s] = (t, i)
+                need[s] = set(range(consumers))
                 full[s].arrive()            # arrive.expect_tx + the TMA bytes landing
                 g += 1
                 yield
 
-    def mma():
+    def release(c, s):
+        need[s].discard(c)
+        empty[s].arrive()
+
+    def consumer(c):
         g = 0
-        for lt, t in enumerate(my_tiles):
-            a, use = lt & 1, lt >> 1
-            if use > 0 and bug != "mma_ignores_acc_empty":
-                while not acc_empty[a].passed((use - 1) & 1):
-                    yield
-            assert acc[a] is None, f"accumulator {a} overwritten before tile {acc[a] and acc[a]['tile']} was drained"
-            acc[a] = {"tile": t, "ks": [], "complete": False}
+        for t in my_tiles:
+            ks, prev = [], None
             for i in range(nkb):
                 s = g % stages
                 while not full[s].passed((g // stages) & 1):
                     yield
-                assert ring[s] == (t, i), f"MMA for ({t},{i}) found {ring[s]} in stage {s}"
-                acc[a]["ks"].append(i)
-                ring[s] = None
-                empty[s].arrive()           # tcgen05.commit
+                assert ring[s] == (t, i), f"MMA of warpgroup {c} for ({t},{i}) found {ring[s]} in stage {s}"
+                assert c in need[s], f"warpgroup {c} reads stage {s} twice"
+                reading[s].add(c)           # wgmma.mma_async x 4 + commit_group
+                ks.append(i)
+                if bug == "consumer_releases_early":
+                    release(c, s)
+                yield
+                if prev is not None:        # wgmma.wait_group 1: the previous stage's group has completed
+                    reading[prev].discard(c)
+                    if bug != "consumer_releases_early":
+                        release(c, prev)
+                prev = s
                 g += 1
                 yield
-            acc[a]["complete"] = True
-            acc_full[a].arrive()
-            yield
+            reading[prev].discard(c)        # wgmma.wait_group 0
+            if bug != "consumer_releases_early":
+                release(c, prev)
+            results[(t, c)] = ks
+            yield                           # the epilogue from registers
 
-    drained = {}
-
-    def epilogue(tid):
-        for lt, t in enumerate(my_tiles):
-            a = lt & 1
-            while not acc_full[a].passed((lt >> 1) & 1):
-                yield
-            assert acc[a] is not None and acc[a]["tile"] == t and acc[a]["complete"], f"epilogue {tid} read accumulator {a} early"
-            snapshot = list(acc[a]["ks"])
-            yield                           # the tcgen05.ld's
-            drained[(t, tid)] = snapshot
-            if sum(1 for k in drained if k[0] == t) == epi_threads:
-                results[t] = snapshot
-                acc[a] = None               # the last reader is done: the stage may be overwritten
-            acc_empty[a].arrive()
-            yield
-
-    roles = [producer(), mma()] + [epilogue(i) for i in range(epi_threads)]
+    roles = [producer()] + [consumer(c) for c in range(consumers)]
     live = list(roles)
     idle_rounds = 0
     while live:
         r = rng.choice(live)
-        before = (tuple(b.phase for b in full + empty + acc_full + acc_empty), tuple(b.pending for b in acc_empty),
-                  len(results), len(drained))
+        before = (tuple(b.phase for b in full + empty), tuple(b.pending for b in empty), len(results))
         try:
             next(r)
         except StopIteration:
             live.remove(r)
             idle_rounds = 0
             continue
-        after = (tuple(b.phase for b in full + empty + acc_full + acc_empty), tuple(b.pending for b in acc_empty),
-                 len(results), len(drained))
+        after = (tuple(b.phase for b in full + empty), tuple(b.pending for b in empty), len(results))
         idle_rounds = idle_rounds + 1 if before == after else 0
         assert idle_rounds < 20000, "dead-lock: no role made progress"
-    assert sorted(results) == my_tiles
-    for t in my_tiles:
-        assert results[t] == list(range(nkb)), f"tile {t} accumulated {results[t]}"
+    assert sorted(results) == sorted((t, c) for t in my_tiles for c in range(consumers))
+    for k, v in results.items():
+        assert v == list(range(nkb)), f"tile/warpgroup {k} accumulated {v}"
     return len(my_tiles)
 
 
@@ -131,7 +122,7 @@ def test_pipeline_protocol_under_random_interleavings(n_tiles, grid, nkb, stages
     assert done == n_tiles          # the CTAs of a launch cover every tile exactly once
 
 
-@pytest.mark.parametrize("bug", ["producer_parity", "producer_never_waits", "mma_ignores_acc_empty"])
+@pytest.mark.parametrize("bug", ["producer_parity", "producer_never_waits", "consumer_releases_early"])
 def test_model_catches_protocol_bugs(bug):
     """Sanity of the model itself: a wrong parity or a missing wait must trip an assertion (or the dead-lock check)
     in at least one interleaving."""

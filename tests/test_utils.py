@@ -97,13 +97,13 @@ def test_config_env_aliases():
 
 def test_device_kernel_bodies_on_an_emulated_grid():
     """csrc/cuda/nn_body.cuh compiled by g++ and walked block by block, thread by thread (csrc/tests/nn_emu_test.cc):
-    the row walk, batch tails, pool index coding and bias-gradient sums of the sm_100a kernels, without a GPU."""
+    the row walk, batch tails, pool index coding and bias-gradient sums of the sm_90a kernels, without a GPU."""
     import subprocess
 
     import bagua_net_b200
 
     root = bagua_net_b200.REPO_ROOT
-    # fused layer kernels; transport executor (copy/reduce/cast/fp8); tcgen05 linear (tiling, TMA boxes, epilogues)
+    # fused layer kernels; transport executor (copy/reduce/cast/fp8); wgmma linear (tiling, TMA boxes, epilogues)
     for name in ("nn_emu_test", "exec_emu_test", "tc_emu_test"):
         subprocess.run(["make", "-s", f"build/tests/{name}"], cwd=root, check=True, capture_output=True)
         r = subprocess.run([os.path.join(root, "build", "tests", name)], capture_output=True, text=True)
@@ -124,7 +124,7 @@ def test_doctor_reports_a_usable_setup_on_cpu():
 
 def test_bench_clock_sampler_with_a_stubbed_nvml(monkeypatch):
     """bench.py samples SM clocks / throttle reasons through NVML every 10 ms inside the timed region; here NVML is a
-    stub (no GPU), on the B200 it is the real library and nvidia-smi stays as the fallback."""
+    stub (no GPU), on the H100 it is the real library and nvidia-smi stays as the fallback."""
     import importlib.util
     import time
     import types
@@ -273,17 +273,17 @@ def _cutlass_include():
     for sp in site.getsitepackages():
         for cand in glob.glob(os.path.join(sp, "*", "data", "cutlass", "include")) + \
                 glob.glob(os.path.join(sp, "*", "3rdparty", "cutlass", "include")):
-            if os.path.exists(os.path.join(cand, "cute", "arch", "mma_sm100_desc.hpp")):
+            if os.path.exists(os.path.join(cand, "cute", "arch", "mma_sm90_desc.hpp")):
                 return cand
     return None
 
 
 def test_tcgen05_descriptors_match_cute_and_plans_are_sane():
-    """The tcgen05 linear kernel (csrc/cuda/tc_gemm.cu) packs its instruction / shared-memory descriptors by hand;
+    """The wgmma linear kernel (csrc/cuda/tc_gemm.cu) packs its shared-memory descriptors by hand;
     csrc/tests/tc_desc_test.cc compares them with the CuTe bit-field definitions and checks the tiling plans."""
     inc = _cutlass_include()
     if inc is None:
-        pytest.skip("no CUTLASS headers with sm100 support in this environment")
+        pytest.skip("no CUTLASS headers with sm90 support in this environment")
     from bagua_net_b200 import LIB_DIR, LIB_NAME
     from bagua_net_b200.utils.native import load
 
@@ -301,15 +301,15 @@ def test_tc_linear_python_plan_and_gating(monkeypatch):
     from bagua_net_b200.ops import tc_linear
 
     monkeypatch.delenv("BNET_TC", raising=False)
-    assert tc_linear.enabled()                           # validated on B200 (profiles/r2): on unless BNET_TC=0 ...
+    assert tc_linear.enabled()                           # on unless BNET_TC=0 ...
     monkeypatch.setenv("BNET_TC", "0")
     assert not tc_linear.enabled()
     monkeypatch.delenv("BNET_TC", raising=False)
     assert not tc_linear.trusted()                       # ... and still only trusted after its self-check passed on a GPU
-    p = tc_linear.plan(32, 4096, 25088)                  # VGG16 fc1 at the flagship batch: weights fill the TMEM lanes
+    p = tc_linear.plan(32, 4096, 25088)                  # VGG16 fc1 at the flagship batch: weights fill the accumulator rows
     assert p["swap"] == 1 and p["bn"] == 32 and p["grid_y"] == 32 and p["k_blocks"] == 392
     p = tc_linear.plan(4096, 4096, 4096, reduce=True, splits=4)
-    assert p["swap"] == 0 and p["bn"] == 256 and p["grid_z"] == 4 and p["k_per_split"] == 16 and p["ctas"] == 37
+    assert p["swap"] == 0 and p["bn"] == 256 and p["grid_z"] == 4 and p["k_per_split"] == 16 and p["ctas"] == 33
     assert p["smem_bytes"] + 1024 <= 227 * 1024
     with pytest.raises(ValueError):
         tc_linear.plan(32, 64, 100)
@@ -317,7 +317,7 @@ def test_tc_linear_python_plan_and_gating(monkeypatch):
 
 
 def test_tc_self_check_runs_isolated_and_is_cached(monkeypatch, tmp_path):
-    """The opt-in tcgen05 path is only trusted after its self-check passed in a CHILD process (a faulting kernel must not
+    """The opt-in wgmma path is only trusted after its self-check passed in a CHILD process (a faulting kernel must not
     poison the trainer's CUDA context); the verdict is cached per library build and GPU model."""
     import glob
 
@@ -326,7 +326,7 @@ def test_tc_self_check_runs_isolated_and_is_cached(monkeypatch, tmp_path):
     from bagua_net_b200.ops import tc_linear
 
     monkeypatch.setenv("BNET_CACHE_DIR", str(tmp_path))
-    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a: "Fake B200")
+    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a: "Fake H100")
     monkeypatch.setattr(torch.cuda, "current_device", lambda: 0)
     assert tc_linear._isolated_self_check(timeout=120) is False        # no GPU in the child either: no verdict, nothing cached
     assert not glob.glob(str(tmp_path / "tc_self_check_*.json"))
@@ -355,9 +355,9 @@ def test_tc_self_check_runs_isolated_and_is_cached(monkeypatch, tmp_path):
 
 
 def test_tc_conv_wgrad_plan_and_gating(monkeypatch, tmp_path):
-    """The tcgen05 filter gradient: every VGG16 layer it accepts (batch 32) is cut into enough pixel slices to put 140+ CTAs
-    on the 148 SMs with one resident CTA each, within shared memory; and the kernel — never run on hardware yet — is only
-    trusted after a self-check in a child process, with the verdict cached under its own name."""
+    """The wgmma filter gradient: every VGG16 layer it accepts (batch 32) is cut into enough pixel slices to put 124+ CTAs
+    on the 132 SMs of an H100 (the library plans for them when it sees no GPU) with one resident CTA each, within shared
+    memory; and the kernel is only trusted after a self-check in a child process, with the verdict cached under its own name."""
     import glob
 
     import torch
@@ -367,7 +367,7 @@ def test_tc_conv_wgrad_plan_and_gating(monkeypatch, tmp_path):
     for cin, cout, hw in ((64, 64, 224), (64, 128, 112), (128, 128, 112), (128, 256, 56), (256, 256, 56), (256, 512, 28), (512, 512, 28),
                           (512, 512, 14)):
         p = tc_conv.wgrad_plan(32, hw, hw, cin, cout)
-        assert 140 <= p["ctas"] * p["grid_z"] <= 148, (cin, cout, hw, p)
+        assert 124 <= p["ctas"] * p["grid_z"] <= 132, (cin, cout, hw, p)
         assert p["k_blocks"] == 32 * hw * hw // 64 and p["k_per_split"] * p["grid_z"] >= p["k_blocks"]          # exact 64-pixel patches
         assert (p["grid_z"] - 1) * p["k_per_split"] < p["k_blocks"]                                              # no empty slice
         assert p["grid_x"] * p["bn"] >= 9 * cin and p["grid_y"] * 128 >= cout and p["smem_bytes"] + 1024 <= 227 * 1024
@@ -384,7 +384,7 @@ def test_tc_conv_wgrad_plan_and_gating(monkeypatch, tmp_path):
     monkeypatch.setattr(tc_conv, "_wgrad_trusted", None)
     monkeypatch.setattr(tc_conv, "usable", lambda: True)
     monkeypatch.setenv("BNET_CACHE_DIR", str(tmp_path))
-    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a: "Fake B200")
+    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a: "Fake H100")
     monkeypatch.setattr(torch.cuda, "current_device", lambda: 0)
     monkeypatch.setattr(torch.cuda, "is_current_stream_capturing", lambda: False)
     monkeypatch.delenv("BNET_TC_WGRAD_BN", raising=False)
@@ -403,7 +403,7 @@ def test_tc_conv_wgrad_plan_and_gating(monkeypatch, tmp_path):
     import bagua_net_b200
 
     lib = os.path.join(bagua_net_b200.LIB_DIR, bagua_net_b200.LIB_NAME)
-    key = f"{os.path.getmtime(lib):.0f}-{os.path.getsize(lib)}-Fake B200-{torch.version.cuda}"
+    key = f"{os.path.getmtime(lib):.0f}-{os.path.getsize(lib)}-Fake H100-{torch.version.cuda}"
     h = hashlib.sha1(key.encode()).hexdigest()[:16]
     json.dump({"ok": False}, open(tmp_path / f"tc_wgrad_self_check_{h}.json", "w"))
     json.dump({"ok": True}, open(tmp_path / f"tc_wgrad_bn128_self_check_{h}.json", "w"))

@@ -272,7 +272,7 @@ def main():
     if a.out:
         os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
         with open(a.out, "w") as f:
-            f.write(f"# CUDA calls issued while a {SPIN_S}s kernel runs on the same device (B200, driver {torch.version.cuda})\n")
+            f.write(f"# CUDA calls issued while a {SPIN_S}s kernel runs on the same device ({torch.cuda.get_device_name()}, CUDA {torch.version.cuda})\n")
             for name, dt, total, verdict, extra in results:
                 f.write(f"{name:52s} {dt:9.2f} ms  {verdict:8s} {extra}\n")
     return 0

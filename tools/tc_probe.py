@@ -1,11 +1,11 @@
-"""First-contact diagnostics for the tcgen05 linear kernel (csrc/cuda/tc_gemm.cu): structured inputs whose products say
+"""First-contact diagnostics for the wgmma linear kernel (csrc/cuda/tc_gemm.cu): structured inputs whose products say
 WHICH part of the data path is wrong when the numerics test fails — instead of "max abs err 3.7".
 
     python tools/tc_probe.py            # prints one verdict per probe; exit code 1 if any failed
 
 Probes (all exact in bf16 / fp32, so any mismatch is a layout or synchronisation bug, not rounding):
-  rows      D[i, j] = i          -> TMEM lane <-> output row mapping of the epilogue warps (lane quarters)
-  cols      D[i, j] = j          -> TMEM column <-> output column mapping, tcgen05.ld register order
+  rows      D[i, j] = i          -> accumulator row <-> output row mapping of the consumer warps
+  cols      D[i, j] = j          -> accumulator column <-> output column mapping, wgmma register order
   kslice    only k in [16s, 16s+16) non-zero, for every s in a 64-wide K block
                                  -> the +32-byte descriptor advance inside the 128-byte swizzle row
   kblock    only K block b non-zero -> ring stage / phase bookkeeping, TMA coordinates
@@ -57,7 +57,7 @@ def run(name, x, w, expect=None, detail=None):
 
 def main():
     if not tc_linear.supported():
-        print("tcgen05 linear unsupported on this device / driver")
+        print("wgmma linear unsupported on this device / driver")
         return 1
     dev = "cuda"
     for (M, N) in ((128, 128), (32, 128)):                  # plain and swapped orientation, one tile each
