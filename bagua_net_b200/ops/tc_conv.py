@@ -49,6 +49,7 @@ def _L():
         _lib.bnet_tc_conv3x3_wgrad.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, i, vp, vp]
         _lib.bnet_tc_conv3x3_wgrad_tiles.argtypes = [i, i]
         _lib.bnet_tc_conv3x3_wgrad_plan.argtypes = [i, i, i, i, i, i, C.POINTER(tc_linear.Plan)]
+        _lib.bnet_tc_conv3x3_plan.argtypes = [i, i, i, i, i, i, C.POINTER(tc_linear.Plan), C.POINTER(C.c_int * 3)]
         _lib.bnet_tc_last_error.restype = C.c_char_p
     return _lib
 
@@ -120,6 +121,17 @@ def wgrad_plan(n: int, h: int, w: int, cin: int, cout: int, splits: int = 0) -> 
     if _L().bnet_tc_conv3x3_wgrad_plan(n, h, w, cin, cout, splits, C.byref(p)) != 0:
         raise ValueError(_L().bnet_tc_last_error().decode())
     return p.as_dict()
+
+
+def conv_plan(n: int, h: int, w: int, cin: int, cout: int, dgrad: bool = False) -> dict:
+    """The tiling ``conv3x3`` (or, with ``dgrad``, ``conv3x3_dgrad``) would use for a layer of cin -> cout channels, plus the
+    patch a 128-row tile covers: ``bw`` x ``bh`` pixels of ``bn_images`` images (``bn`` is the tile width in output channels,
+    as in ``tc_linear.plan``).  Host-only; works without a GPU."""
+    p, patch = tc_linear.Plan(), (C.c_int * 3)()
+    red, cols = (cout, cin) if dgrad else (cin, cout)
+    if _L().bnet_tc_conv3x3_plan(n, h, w, red, cols, 1 if dgrad else 0, C.byref(p), C.byref(patch)) != 0:
+        raise ValueError(_L().bnet_tc_last_error().decode())
+    return dict(p.as_dict(), bw=patch[0], bh=patch[1], bn_images=patch[2])
 
 
 _wgrad_scratch: dict = {}

@@ -107,14 +107,16 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _auto_splits(M: int, N: int, K: int) -> int:
+def _auto_splits(M: int, N: int, K: int, sms: int | None = None) -> int:
     """Small-batch layers are weight streaming: with M <= 64 a [M, N] output has only N / 128 tiles — 32 CTAs for the VGG
     classifier — and one SM cannot pull its 128 x K weight slab at more than a fraction of HBM speed.  Splitting K over
-    grid.z puts every SM to work; the partial tiles meet as fp32 adds in a small workspace."""
+    grid.z puts every SM to work; the partial tiles meet as fp32 adds in a small workspace.  ``sms``: the SM count to plan
+    for (default: the current device's)."""
     if M > 64 or K < 2048:
         return 1
     tiles = (N + 127) // 128
-    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    if sms is None:
+        sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
     return max(1, min(8, sms // max(tiles, 1), K // 1024))
 
 
@@ -248,7 +250,7 @@ class _LinearAct(torch.autograd.Function):
     def backward(ctx, gy):
         x, w, y = ctx.saved_tensors
         if ctx.relu:
-            gy = gy * (y > 0).to(gy.dtype)
+            gy = gy.masked_fill(y <= 0, 0)          # torch's threshold_backward: a NaN output passes its gradient
         gy = gy.contiguous()
         tc = _bwd_on_tc(gy, x, w)
         gx = gw = None

@@ -97,6 +97,11 @@ template <typename T> BNET_HD void store_raw_stream(T* p, const typename Vec<T>:
   st_stream(reinterpret_cast<typename Vec<T>::Raw*>(p), v);
 }
 
+// ---- ReLU as eager torch computes it: relu(NaN) = NaN (fmaxf would return 0 and hide a diverged run), and the backward
+// passes the gradient unless y <= 0 (threshold_backward), so a NaN activation passes it too
+BNET_HD float relu(float v) { return v <= 0.f ? 0.f : v; }
+BNET_HD bool relu_passes(float y) { return !(y <= 0.f); }
+
 // ---- y = relu(z + b), in place ---------------------------------------------------------------------------------
 // gtid/gthreads: global thread index / number of threads in the grid.  nvec = rows * cvec 16-byte vectors.
 template <typename T>
@@ -107,13 +112,15 @@ BNET_HD void bias_relu_thread(T* z, const T* bias, size_t nvec, int cvec, size_t
     Vec<T>::unpack(load_raw(z + i * V), v);
     Vec<T>::unpack(load_raw(bias + (i % cvec) * V), b);
 #pragma unroll
-    for (int k = 0; k < V; k++) v[k] = fmaxf(v[k] + b[k], 0.f);
+    for (int k = 0; k < V; k++) v[k] = relu(v[k] + b[k]);
     store_raw(z + i * V, Vec<T>::pack(v));
   }
 }
 
 // ---- p = maxpool2x2(relu(z + b)) with a 1-byte code per element ------------------------------------------------
-// code: bits 0-1 = position of the max inside the window (dy*2+dx), bit 2 = max > 0 (gradient flows)
+// code: bits 0-1 = position of the max inside the window (dy*2+dx), bit 2 = the gradient flows (relu_passes(max)).
+// The window follows torch's max_pool2d: the first maximum wins a tie, and a NaN wins over any number (a later NaN over an
+// earlier one), so the pooled value is NaN and the gradient goes to that element.
 template <typename T>
 BNET_HD void bias_relu_pool_fwd_thread(const T* z, const T* bias, T* p, uint8_t* idx, int N, int H, int W, int cvec,
                                        size_t gtid, size_t gthreads) {
@@ -142,21 +149,22 @@ BNET_HD void bias_relu_pool_fwd_thread(const T* z, const T* bias, T* p, uint8_t*
     uint8_t* code = reinterpret_cast<uint8_t*>(&codes);
 #pragma unroll
     for (int k = 0; k < V; k++) {
-      float m = v[0][k];
+      float m = v[0][k] + b[k];
       int a = 0;
 #pragma unroll
-      for (int q = 1; q < 4; q++)
-        if (v[q][k] > m) { m = v[q][k]; a = q; }
-      m += b[k];
-      out[k] = fmaxf(m, 0.f);
-      code[k] = (uint8_t)(a | (m > 0.f ? 4 : 0));
+      for (int q = 1; q < 4; q++) {
+        const float u = v[q][k] + b[k];
+        if (u > m || u != u) { m = u; a = q; }
+      }
+      out[k] = relu(m);
+      code[k] = (uint8_t)(a | (relu_passes(m) ? 4 : 0));
     }
     store_raw(p + i * V, Vec<T>::pack(out));
     *reinterpret_cast<typename Vec<T>::Code*>(idx + i * V) = codes;
   }
 }
 
-// ---- gz = gy * (y > 0) ; acc += this thread's column sums of gz -------------------------------------------------
+// ---- gz = relu_passes(y) ? gy : 0 ; acc += this thread's column sums of gz -------------------------------------------------
 // rows = N*H*W, cvec = C / V.  The block owns rpb = threads/cvec consecutive rows per step; thread (trow, grp)
 // always sees channel group grp.  U rows per thread are loaded (2*U 16-byte requests in flight) before any
 // dependent work; out-of-range rows of the last batch re-read row r0 (valid) instead of branching.
@@ -184,7 +192,7 @@ BNET_HD void relu_bwd_thread(const T* gy, const T* y, T* gz, size_t rows, int cv
         Vec<T>::unpack(a[u], af);
 #pragma unroll
         for (int k = 0; k < V; k++) {
-          gf[k] = af[k] > 0.f ? gf[k] : 0.f;
+          gf[k] = relu_passes(af[k]) ? gf[k] : 0.f;
           acc[k] += gf[k];
         }
         store_raw_stream(gz + (r * cvec + grp) * V, Vec<T>::pack(gf));
@@ -247,7 +255,7 @@ BNET_HD void pool_relu_bwd_thread(const T* gp, const uint8_t* idx, T* gz, int N,
 //   forward : z = conv(x, w)                         (library call)
 //             stats  = per-channel sum, sum of squares of z                                 (bn_stats, 1 read)
 //             y      = relu?( (z - mean) * invstd * gamma + beta  (+ residual) )            (bn_apply, 1-2 reads, 1 write)
-//   backward: dy     = relu? gy * (y > 0) : gy
+//   backward: dy     = relu? (relu_passes(y) ? gy : 0) : gy
 //             s1, s2 = per-channel sum of dy, of dy * xhat        (xhat = (z - mean) * invstd)  (bn_bwd_reduce)
 //             gz     = gamma * invstd * (dy - s1/M - xhat * s2/M) ;  gres = dy              (bn_bwd_apply)
 // Same thread/row mapping as relu_bwd_thread: thread (trow, grp) always sees channel group grp, so its channel
@@ -328,7 +336,7 @@ BNET_HD void bn_apply_thread(const T* z, const T* res, T* y, size_t rows, int cv
         for (int k = 0; k < V; k++) {
           float v = f[k] * scale[k] + shift[k];
           if (res) v += q[k];
-          f[k] = relu ? fmaxf(v, 0.f) : v;
+          f[k] = relu ? bnet::nn::relu(v) : v;
         }
         store_raw_stream(y + (r * cvec + grp) * V, Vec<T>::pack(f));
       }
@@ -362,7 +370,7 @@ BNET_HD void bn_bwd_reduce_thread(const T* gy, const T* y, const T* z, size_t ro
         if (relu) Vec<T>::unpack(yr[u], a);
 #pragma unroll
         for (int k = 0; k < V; k++) {
-          const float dy = (!relu || a[k] > 0.f) ? g[k] : 0.f;
+          const float dy = (!relu || relu_passes(a[k])) ? g[k] : 0.f;
           acc[k] += dy;
           acc[V + k] += dy * ((f[k] - mean[k]) * invstd[k]);
         }
@@ -399,7 +407,7 @@ BNET_HD void bn_bwd_apply_thread(const T* gy, const T* y, const T* z, T* gz, T* 
         if (relu) Vec<T>::unpack(yr[u], act);
 #pragma unroll
         for (int k = 0; k < V; k++) {
-          const float dy = (!relu || act[k] > 0.f) ? g[k] : 0.f;
+          const float dy = (!relu || relu_passes(act[k])) ? g[k] : 0.f;
           g[k] = dy;
           o[k] = a[k] * (dy - c1[k] - (f[k] - mean[k]) * invstd[k] * c2[k]);
         }

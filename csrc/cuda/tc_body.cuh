@@ -519,7 +519,7 @@ BNET_TC_HD void epilogue_chunk(const TcArgs& args, int i_glob, int j0, const flo
   for (int u = 0; u < 16; u++) {
     const float b = kSwap ? bias_i : ((add_bias && j0 + u < args.rows_b) ? bf16_to_f32(args.bias[j0 + u]) : 0.f);
     f[u] = acc[u] + b;
-    if (!kReduce && args.act == BNET_TC_ACT_RELU) f[u] = f[u] > 0.f ? f[u] : 0.f;
+    if (!kReduce && args.act == BNET_TC_ACT_RELU) f[u] = f[u] <= 0.f ? 0.f : f[u];     // (eager torch: relu(NaN) = NaN)
   }
   if (!kReduce) {
     uint16_t* o = static_cast<uint16_t*>(args.outs[0]);

@@ -739,6 +739,23 @@ BNET_API int bnet_tc_conv3x3_wgrad(const void* gy, const void* x, void* dw, floa
   return run_conv_wgrad(gy, x, dw, ws, counters, N, H, W, Cin, Cout, splits, err_dev, stream);
 }
 BNET_API int bnet_tc_conv3x3_wgrad_tiles(int Cin, int Cout) { return wgrad_max_tiles(Cin, Cout); }
+// the tiling of a 3x3 convolution (pure host function, like bnet_tc_plan): Cred / Cn as bnet_tc_conv3x3 (forward: Cin / Cout) or
+// bnet_tc_conv3x3_dgrad (dgrad = 1: Cout / Cin) passes them to setup_conv; patch = {bw, bh, bn}, the pixels of one 128-row tile
+BNET_API int bnet_tc_conv3x3_plan(int N, int H, int W, int Cred, int Cn, int dgrad, BnetTcPlan* plan, int patch[3]) {
+  if (!plan || !patch) { g_err = "null plan"; return -1; }
+  ConvProblem cp;
+  uint16_t dummy[8] = {};
+  int err_dummy = 0;
+  if (const char* e = setup_conv(dummy, dummy, nullptr, dummy, N, H, W, Cred, Cn, BNET_TC_ACT_NONE, dgrad, &err_dummy, sm_count(), &cp)) {
+    g_err = e;
+    return -1;
+  }
+  *plan = cp.plan;
+  patch[0] = cp.args.conv.bw;
+  patch[1] = cp.args.conv.bh;
+  patch[2] = cp.args.conv.bn;
+  return 0;
+}
 // the tiling of a filter gradient (pure host function, like bnet_tc_plan): grid_x x grid_y tiles of 128 x bn, grid_z slices of
 // the k_blocks 64-pixel blocks, ctas per slice
 BNET_API int bnet_tc_conv3x3_wgrad_plan(int N, int H, int W, int Cin, int Cout, int splits, BnetTcPlan* plan) {

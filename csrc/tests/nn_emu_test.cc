@@ -42,25 +42,50 @@ template <> struct Conv<__nv_bfloat16> {
 };
 
 template <typename T> static bool same(T a, T b) { return memcmp(&a, &b, sizeof(T)) == 0; }
+// equal bits, or both NaN (a NaN's payload is not part of the contract)
+template <typename T> static bool same_or_nan(T a, T b) {
+  const float fa = Conv<T>::from(a), fb = Conv<T>::from(b);
+  return same(a, b) || (fa != fa && fb != fb);
+}
+
+// torch's rules: relu(x) = x <= 0 ? 0 : x (NaN stays NaN); threshold_backward(g, y) = y <= 0 ? 0 : g (a NaN y passes g)
+static float relu_ref(float x) { return x <= 0.f ? 0.f : x; }
+static bool passes_ref(float y) { return !(y <= 0.f); }
+
+// with `specials`, every 5th element of a tensor is NaN, +Inf, -Inf or -0 instead (what a diverged run feeds a layer)
+static float special(size_t i) {
+  static const float v[4] = {NAN, INFINITY, -INFINITY, -0.0f};
+  return v[(i / 5) % 4];
+}
+template <typename T> static void sprinkle(std::vector<T>& t, size_t phase) {
+  for (size_t i = phase % 5; i < t.size(); i += 5) t[i] = Conv<T>::to(special(i + phase));
+}
+// sums that hold a NaN on both sides agree
+static bool close_sum(double got, double want) {
+  if (got != got || want != want) return got != got && want != want;
+  if (isinf(got) || isinf(want)) return got == want;
+  return fabs(got - want) <= 1e-3 * (1.0 + fabs(want));
+}
 
 template <typename T>
-static void test_bias_relu(size_t rows, int C, int nblocks) {
+static void test_bias_relu(size_t rows, int C, int nblocks, bool specials = false) {
   constexpr int V = Vec<T>::N;
   const int cvec = C / V;
   std::vector<T> z(rows * C), z0, bias(C);
   for (auto& v : z) v = Conv<T>::to(frand());
   for (auto& v : bias) v = Conv<T>::to(frand() * 0.5f);
+  if (specials) { sprinkle(z, 0); sprinkle(bias, 3); }
   z0 = z;
   const size_t gthreads = (size_t)nblocks * 256;
   for (size_t t = 0; t < gthreads; t++) bias_relu_thread<T>(z.data(), bias.data(), rows * cvec, cvec, t, gthreads);
   for (size_t i = 0; i < rows * C; i++) {
-    float e = fmaxf(Conv<T>::from(z0[i]) + Conv<T>::from(bias[i % C]), 0.f);
-    CHECK(same(z[i], Conv<T>::to(e)), "%s bias_relu rows=%zu C=%d i=%zu", Conv<T>::name(), rows, C, i);
+    float e = relu_ref(Conv<T>::from(z0[i]) + Conv<T>::from(bias[i % C]));
+    CHECK(same_or_nan(z[i], Conv<T>::to(e)), "%s bias_relu rows=%zu C=%d i=%zu", Conv<T>::name(), rows, C, i);
   }
 }
 
 template <typename T>
-static void test_relu_bwd(size_t rows, int C, int nblocks) {
+static void test_relu_bwd(size_t rows, int C, int nblocks, bool specials = false) {
   constexpr int V = Vec<T>::N;
   const int cvec = C / V;
   const int threads = (256 / cvec) * cvec, rpb = threads / cvec;
@@ -70,6 +95,7 @@ static void test_relu_bwd(size_t rows, int C, int nblocks) {
     float a = frand();
     y[i] = Conv<T>::to(a > 0.3f ? a : 0.f);     // post-ReLU activations: many exact zeros
   }
+  if (specials) { sprinkle(y, 0); sprinkle(gy, 2); }
   memset((void*)gz.data(), 0x7f, gz.size() * sizeof(T));   // sentinel: every element must be overwritten
   std::vector<double> gb(C, 0.0);
   for (int b = 0; b < nblocks; b++)
@@ -81,16 +107,16 @@ static void test_relu_bwd(size_t rows, int C, int nblocks) {
     }
   std::vector<double> ref(C, 0.0);
   for (size_t i = 0; i < rows * C; i++) {
-    float e = Conv<T>::from(y[i]) > 0.f ? Conv<T>::from(gy[i]) : 0.f;
-    CHECK(same(gz[i], Conv<T>::to(e)), "%s relu_bwd rows=%zu C=%d blocks=%d i=%zu", Conv<T>::name(), rows, C, nblocks, i);
+    float e = passes_ref(Conv<T>::from(y[i])) ? Conv<T>::from(gy[i]) : 0.f;
+    CHECK(same_or_nan(gz[i], Conv<T>::to(e)), "%s relu_bwd rows=%zu C=%d blocks=%d i=%zu", Conv<T>::name(), rows, C, nblocks, i);
     ref[i % C] += e;
   }
   for (int c = 0; c < C; c++)
-    CHECK(fabs(gb[c] - ref[c]) <= 1e-3 * (1.0 + fabs(ref[c])), "%s relu_bwd bias grad c=%d %f vs %f", Conv<T>::name(), c, gb[c], ref[c]);
+    CHECK(close_sum(gb[c], ref[c]), "%s relu_bwd bias grad c=%d %f vs %f", Conv<T>::name(), c, gb[c], ref[c]);
 }
 
 template <typename T>
-static void test_pool(int N, int H, int W, int C, int nblocks) {
+static void test_pool(int N, int H, int W, int C, int nblocks, bool specials = false) {
   constexpr int V = Vec<T>::N;
   const int cvec = C / V, Ho = H / 2, Wo = W / 2;
   const size_t in = (size_t)N * H * W * C, out = (size_t)N * Ho * Wo * C;
@@ -99,6 +125,15 @@ static void test_pool(int N, int H, int W, int C, int nblocks) {
   for (auto& v : z) v = Conv<T>::to(frand());
   for (auto& v : bias) v = Conv<T>::to(frand() * 0.5f);
   for (auto& v : gp) v = Conv<T>::to(frand());
+  if (specials) {
+    sprinkle(z, 1);
+    bias[0] = Conv<T>::to(NAN);
+    if (C > 1) bias[1] = Conv<T>::to(INFINITY);
+    if (C > 2) bias[2] = Conv<T>::to(-INFINITY);
+    // exact ties inside windows (the first maximum wins) and windows with two NaNs (the last one wins)
+    for (size_t i = 0; i + 3 * C < in; i += 7 * C + 1) z[i + C] = z[i];
+    for (size_t i = 2; i + (size_t)W * C < in; i += 11 * C + 3) { z[i] = Conv<T>::to(NAN); z[i + (size_t)W * C] = Conv<T>::to(NAN); }
+  }
   // ---- forward
   const size_t gthreads = (size_t)nblocks * 256;
   for (size_t t = 0; t < gthreads; t++)
@@ -108,16 +143,18 @@ static void test_pool(int N, int H, int W, int C, int nblocks) {
     for (int ho = 0; ho < Ho; ho++)
       for (int wo = 0; wo < Wo; wo++)
         for (int c = 0; c < C; c++) {
-          float m = Conv<T>::from(z[at(n, 2 * ho, 2 * wo, c)]);
+          // torch's max_pool2d: the first maximum wins a tie, a NaN wins over any number (the last NaN over an earlier one)
+          const float b = Conv<T>::from(bias[c]);
+          float m = Conv<T>::from(z[at(n, 2 * ho, 2 * wo, c)]) + b;
           int a = 0;
           for (int q = 1; q < 4; q++) {
-            float v = Conv<T>::from(z[at(n, 2 * ho + q / 2, 2 * wo + q % 2, c)]);
-            if (v > m) { m = v; a = q; }
+            float v = Conv<T>::from(z[at(n, 2 * ho + q / 2, 2 * wo + q % 2, c)]) + b;
+            if (v > m || v != v) { m = v; a = q; }
           }
-          m += Conv<T>::from(bias[c]);
           size_t o = (((size_t)n * Ho + ho) * Wo + wo) * C + c;
-          CHECK(same(p[o], Conv<T>::to(fmaxf(m, 0.f))), "%s pool fwd value o=%zu", Conv<T>::name(), o);
-          CHECK(idx[o] == (uint8_t)(a | (m > 0.f ? 4 : 0)), "%s pool fwd code o=%zu got %u", Conv<T>::name(), o, idx[o]);
+          CHECK(same_or_nan(p[o], Conv<T>::to(relu_ref(m))), "%s pool fwd value o=%zu", Conv<T>::name(), o);
+          CHECK(idx[o] == (uint8_t)(a | (passes_ref(m) ? 4 : 0)), "%s pool fwd code o=%zu got %u want %u", Conv<T>::name(), o, idx[o],
+                (unsigned)(a | (passes_ref(m) ? 4 : 0)));
         }
   // ---- backward through the codes
   const int threads = (256 / cvec) * cvec, rpb = threads / cvec;
@@ -140,12 +177,12 @@ static void test_pool(int N, int H, int W, int C, int nblocks) {
           ref[c] += g;
           for (int q = 0; q < 4; q++) {
             float e = ((idx[o] & 3) == q) ? g : 0.f;
-            CHECK(same(gz[at(n, 2 * ho + q / 2, 2 * wo + q % 2, c)], Conv<T>::to(e)), "%s pool bwd N=%d H=%d W=%d C=%d o=%zu q=%d",
+            CHECK(same_or_nan(gz[at(n, 2 * ho + q / 2, 2 * wo + q % 2, c)], Conv<T>::to(e)), "%s pool bwd N=%d H=%d W=%d C=%d o=%zu q=%d",
                   Conv<T>::name(), N, H, W, C, o, q);
           }
         }
   for (int c = 0; c < C; c++)
-    CHECK(fabs(gb[c] - ref[c]) <= 1e-3 * (1.0 + fabs(ref[c])), "%s pool bwd bias grad c=%d %f vs %f", Conv<T>::name(), c, gb[c], ref[c]);
+    CHECK(close_sum(gb[c], ref[c]), "%s pool bwd bias grad c=%d %f vs %f", Conv<T>::name(), c, gb[c], ref[c]);
 }
 
 template <typename T>
@@ -235,7 +272,7 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
     }
   for (size_t i = 0; i < rows * C; i++) {
     const int c = (int)(i % C);
-    double dy = (!relu || Conv<T>::from(y[i]) > 0.f) ? Conv<T>::from(gy[i]) : 0.0;
+    double dy = (!relu || passes_ref(Conv<T>::from(y[i]))) ? Conv<T>::from(gy[i]) : 0.0;
     r1[c] += dy;
     r2[c] += dy * (Conv<T>::from(z[i]) - mean[c]) * invstd[c];
   }
@@ -263,13 +300,50 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
   const double tol_g = bf ? 2e-2 : 5e-4;
   for (size_t i = 0; i < rows * C; i++) {
     const int c = (int)(i % C);
-    double dy = (!relu || Conv<T>::from(y[i]) > 0.f) ? Conv<T>::from(gy[i]) : 0.0;
+    double dy = (!relu || passes_ref(Conv<T>::from(y[i]))) ? Conv<T>::from(gy[i]) : 0.0;
     double xhat = (Conv<T>::from(z[i]) - mean[c]) * invstd[c];
     double want = Conv<T>::from(gamma[c]) * invstd[c] * (dy - r1[c] / rows - xhat * r2[c] / rows);
     CHECK(fabs(Conv<T>::from(gz[i]) - want) <= tol_g * (1.0 + fabs(want)), "%s bn bwd rows=%zu C=%d i=%zu got %f want %f", Conv<T>::name(),
           rows, C, i, Conv<T>::from(gz[i]), want);
     if (with_res) CHECK(same(gres[i], Conv<T>::to((float)dy)), "%s bn gres i=%zu", Conv<T>::name(), i);
   }
+}
+
+// BatchNorm apply / backward with ReLU on activations holding NaN and +-Inf: scale 1, shift 0 makes y = relu(z), and the
+// backward passes dy wherever torch's threshold_backward would (y NaN included)
+template <typename T>
+static void test_bn_specials(size_t rows, int C) {
+  constexpr int V = Vec<T>::N;
+  const int cvec = C / V, threads = (256 / cvec) * cvec, rpb = threads / cvec;
+  std::vector<T> z(rows * C), y(rows * C), gy(rows * C), gz(rows * C), gres(rows * C);
+  for (size_t i = 0; i < rows * C; i++) { z[i] = Conv<T>::to(frand()); gy[i] = Conv<T>::to(frand()); }
+  sprinkle(z, 0);
+  float one[V], zero[V];
+  for (int k = 0; k < V; k++) { one[k] = 1.f; zero[k] = 0.f; }
+  memset((void*)y.data(), 0x7f, y.size() * sizeof(T));
+  for (int t = 0; t < threads; t++)
+    bn_apply_thread<T, 4>(z.data(), nullptr, y.data(), rows, cvec, rpb, t % cvec, t / cvec, 0, 1, one, zero, true);
+  for (size_t i = 0; i < rows * C; i++)
+    CHECK(same_or_nan(y[i], Conv<T>::to(relu_ref(Conv<T>::from(z[i])))), "%s bn apply relu i=%zu", Conv<T>::name(), i);
+  // mean 0, invstd 1, a 1, c1 = c2 = 0: gz = dy - z * 0, and gres = dy
+  std::vector<double> s1(C, 0.0);
+  for (int t = 0; t < threads; t++) {
+    float acc[2 * V];
+    for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
+    bn_bwd_reduce_thread<T, 2>(gy.data(), y.data(), z.data(), rows, cvec, rpb, t % cvec, t / cvec, 0, 1, zero, one, true, acc);
+    for (int k = 0; k < V; k++) s1[(t % cvec) * V + k] += acc[k];
+    bn_bwd_apply_thread<T, 2>(gy.data(), y.data(), z.data(), gz.data(), gres.data(), rows, cvec, rpb, t % cvec, t / cvec, 0, 1, zero, one,
+                              one, zero, zero, true);
+  }
+  std::vector<double> r1(C, 0.0);
+  for (size_t i = 0; i < rows * C; i++) {
+    const float dy = passes_ref(Conv<T>::from(y[i])) ? Conv<T>::from(gy[i]) : 0.f;
+    r1[i % C] += dy;
+    CHECK(same_or_nan(gres[i], Conv<T>::to(dy)), "%s bn bwd gres i=%zu", Conv<T>::name(), i);
+    const float want = dy - Conv<T>::from(z[i]) * 0.f;     // xhat * c2: NaN where z is not finite
+    CHECK(same_or_nan(gz[i], Conv<T>::to(want)), "%s bn bwd gz i=%zu", Conv<T>::name(), i);
+  }
+  for (int c = 0; c < C; c++) CHECK(close_sum(s1[c], r1[c]), "%s bn bwd s1 c=%d", Conv<T>::name(), c);
 }
 
 template <typename T>
@@ -308,9 +382,22 @@ static void run_all() {
   }
 }
 
+// NaN / +-Inf in the inputs: the layers follow eager torch (NaN propagates through ReLU and wins a pooling window)
+template <typename T>
+static void run_specials() {
+  constexpr int V = Vec<T>::N;
+  test_bias_relu<T>(257, 8 * V, 3, true);
+  test_relu_bwd<T>(257, 8 * V, 3, true);
+  test_pool<T>(2, 6, 10, 8 * V, 3, true);
+  test_pool<T>(3, 8, 8, 64, 2, true);
+  test_bn_specials<T>(100, 8 * V);
+}
+
 int main() {
   run_all<float>();
   run_all<__nv_bfloat16>();
+  run_specials<float>();
+  run_specials<__nv_bfloat16>();
   printf("%s (%d failure%s)\n", g_fail ? "FAILED" : "nn kernel emulation tests passed", g_fail, g_fail == 1 ? "" : "s");
   return g_fail ? 1 : 0;
 }

@@ -490,7 +490,36 @@ static void conv_wgrad(int N, int H, int W, int Cin, int Cout, int sms, int spli
         N, H, W, Cin, Cout, wp.args.conv.bw, wp.args.conv.bh, wp.args.conv.bn, wp.plan.bn, wp.args.n_tiles, wp.plan.grid_z, wp.plan.ctas, bad, dirty);
 }
 
+// The fused ReLU of the epilogue on NaN / +-Inf accumulators, both orientations, vector and scalar stores: eager torch's
+// relu(NaN) = NaN, relu(+Inf) = +Inf, relu(-Inf) = relu(-0) = 0
+static void epilogue_specials() {
+  const float sp[8] = {NAN, INFINITY, -INFINITY, -0.0f, 1.5f, -2.0f, 0.0f, 300.0f};
+  for (int swap = 0; swap < 2; swap++)
+    for (int cols : {16, 13}) {                          // 16: one 16-element vector store; 13: the scalar path
+      std::vector<uint16_t> buf(64 * 32 + 16, 0xdead);
+      uint16_t* o = buf.data();
+      while (reinterpret_cast<uintptr_t>(o) & 15) o++;
+      TcArgs a;
+      memset(&a, 0, sizeof(a));
+      a.rows_a = 4; a.rows_b = cols; a.ldo = 32; a.act = BNET_TC_ACT_RELU; a.outs[0] = o; a.n_outs = 1;
+      for (int i = 0; i < a.rows_a; i++) {
+        float acc[16];
+        for (int u = 0; u < 16; u++) acc[u] = sp[(u + i) % 8];
+        if (swap) epilogue_chunk<true, false>(a, i, 0, acc, false, HostOut{});
+        else epilogue_chunk<false, false>(a, i, 0, acc, false, HostOut{});
+        for (int u = 0; u < cols; u++) {
+          const float v = acc[u], want = v <= 0.f ? 0.f : v;
+          const uint16_t got = swap ? o[size_t(u) * a.ldo + i] : o[size_t(i) * a.ldo + u];
+          const float g = bf16_to_f32(got);
+          CHECK(want != want ? g != g : (g == want && !(got & 0x8000)), "relu epilogue swap=%d cols=%d: relu(%f) gave %f (0x%04x)", swap,
+                cols, v, g, got);
+        }
+      }
+    }
+}
+
 int main() {
+  epilogue_specials();
   // filter gradients: exact and ragged 64-pixel patches, Cout below / above one lane tile, tiles that straddle taps (Cin = 64
   // with 128 columns), columns past 9 * Cin (Cin = 128 with 256-column tiles), one slice / many slices / persistent CTAs
   conv_wgrad(2, 8, 8, 64, 64, 132, 0);

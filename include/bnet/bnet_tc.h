@@ -98,6 +98,9 @@ int bnet_tc_conv3x3_wgrad(const void* gy, const void* x, void* dw, float* ws, in
                           int splits, int* err_dev, void* stream);
 int bnet_tc_conv3x3_wgrad_tiles(int Cin, int Cout);
 int bnet_tc_conv3x3_wgrad_plan(int N, int H, int W, int Cin, int Cout, int splits, BnetTcPlan* plan);   /* host only */
+/* The tiling of bnet_tc_conv3x3 (dgrad = 0: Cred = Cin, Cn = Cout) or bnet_tc_conv3x3_dgrad (dgrad = 1: Cred = Cout, Cn = Cin);
+ * patch = {bw, bh, bn}: one 128-row tile is bw x bh pixels of bn images.  Host only. */
+int bnet_tc_conv3x3_plan(int N, int H, int W, int Cred, int Cn, int dgrad, BnetTcPlan* plan, int patch[3]);
 
 /* The 64-bit wgmma shared-memory matrix descriptor (K-major, 128-byte swizzle) the kernel issues, exposed so a host test
  * can compare it with the CuTe definition. */
