@@ -6,8 +6,9 @@ convolution is folded into one sm_90a pass in forward and one in backward.
 
 The convolution itself stays a library call (cuDNN implicit GEMM on the tensor cores); the bias
 add, ReLU, 2x2 max-pool, their backward passes and the bias-gradient reduction are ours.
-Inputs must be channels_last with C_out a multiple of 8 (bf16) / 4 (fp32); otherwise the layer
-falls back to the eager PyTorch ops.
+Inputs must be channels_last with C_out a multiple of 8 (bf16) / 4 (fp32) and at most 256 such 16-byte
+channel groups (2048 bf16 / 1024 fp32 channels, the widest the reduce kernels take); otherwise the layer falls
+back to the eager PyTorch ops.
 """
 from __future__ import annotations
 
@@ -62,7 +63,10 @@ def _nhwc(t: torch.Tensor) -> bool:
 
 
 def _supported(x: torch.Tensor, cout: int) -> bool:
-    return x.is_cuda and x.dtype in _DT and cout % (8 if x.dtype == torch.bfloat16 else 4) == 0
+    """Can the fused kernels take a layer with `cout` output channels: whole 16-byte channel vectors, and at most 256 of them
+    per pixel (a block of the backward and BatchNorm reductions holds one row of them)."""
+    vec = 8 if x.dtype == torch.bfloat16 else 4
+    return x.is_cuda and x.dtype in _DT and cout % vec == 0 and cout // vec <= 256
 
 
 def _conv(x, w, stride, padding):
@@ -271,8 +275,7 @@ def conv_bn_act(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d, relu: bool
     kernels (statistics, normalise + affine + residual + ReLU in one pass, two-kernel backward); anything else
     (eval mode, exotic configurations) takes the eager PyTorch chain."""
     c = conv.out_channels
-    vec = 8 if x.dtype == torch.bfloat16 else 4
-    if (bn.training and _supported(x, c) and c // vec <= 256 and conv.bias is None and conv.groups == 1
+    if (bn.training and _supported(x, c) and conv.bias is None and conv.groups == 1
             and conv.dilation == (1, 1) and bn.affine and bn.track_running_stats and bn.momentum is not None
             and bn.weight.dtype == x.dtype and bn.running_mean.dtype == x.dtype):
         if not _nhwc(x):

@@ -253,7 +253,7 @@ BNET_HD void pool_relu_bwd_thread(const T* gp, const uint8_t* idx, T* gz, int N,
 
 // ==== training-mode BatchNorm fused with what follows it in a ResNet block ===========================================
 //   forward : z = conv(x, w)                         (library call)
-//             stats  = per-channel sum, sum of squares of z                                 (bn_stats, 1 read)
+//             stats  = per-channel sum, sum of squares of z - K, K = z[row 0]               (bn_stats, 1 read)
 //             y      = relu?( (z - mean) * invstd * gamma + beta  (+ residual) )            (bn_apply, 1-2 reads, 1 write)
 //   backward: dy     = relu? (relu_passes(y) ? gy : 0) : gy
 //             s1, s2 = per-channel sum of dy, of dy * xhat        (xhat = (z - mean) * invstd)  (bn_bwd_reduce)
@@ -261,16 +261,26 @@ BNET_HD void pool_relu_bwd_thread(const T* gp, const uint8_t* idx, T* gz, int N,
 // Same thread/row mapping as relu_bwd_thread: thread (trow, grp) always sees channel group grp, so its channel
 // constants live in registers for the whole walk.
 
-// mean / inverse standard deviation of this thread's V channels from the accumulated sums (biased variance)
+// The statistics are sums of d = z - K with a per-channel pivot K, the channel's value in row 0.  Plain sums of z and z^2
+// would give var = E[z^2] - mean^2, whose fp32 rounding error grows as (mean / std)^2 * 2^-24 (0.4 relative at
+// mean / std = 1024); d is of the order of std, so var = E[d^2] - E[d]^2 keeps its error near 2^-24 at any offset.
+// A NaN or infinite pivot makes every d, and so the channel's statistics, NaN (as eager torch's are).
+template <typename T> BNET_HD void bn_pivot(const T* z, int grp, float* pivot) {
+  Vec<T>::unpack(load_raw(z + (size_t)grp * Vec<T>::N), pivot);
+}
+
+// mean / inverse standard deviation of this thread's V channels from the shifted sums (biased variance); a NaN variance
+// stays NaN (the clamp only lifts a rounding-negative value to 0)
 template <int V>
-BNET_HD void bn_moments(const float* stats, int C, int grp, float inv_m, float eps, float* mean, float* invstd, float* var) {
+BNET_HD void bn_moments(const float* stats, const float* pivot, int C, int grp, float inv_m, float eps, float* mean, float* invstd,
+                        float* var) {
 #pragma unroll
   for (int k = 0; k < V; k++) {
     const int c = grp * V + k;
-    const float m = stats[c] * inv_m;
-    float v = stats[C + c] * inv_m - m * m;
-    v = v > 0.f ? v : 0.f;
-    mean[k] = m;
+    const float d = stats[c] * inv_m;
+    float v = stats[C + c] * inv_m - d * d;
+    v = v < 0.f ? 0.f : v;
+    mean[k] = pivot[k] + d;
     var[k] = v;
 #if defined(__CUDA_ARCH__)
     invstd[k] = rsqrtf(v + eps);
@@ -280,10 +290,10 @@ BNET_HD void bn_moments(const float* stats, int C, int grp, float inv_m, float e
   }
 }
 
-// acc[0..V) += z ; acc[V..2V) += z*z
+// acc[0..V) += z - pivot ; acc[V..2V) += (z - pivot)^2
 template <typename T, int U>
 BNET_HD void bn_stats_thread(const T* z, size_t rows, int cvec, int rpb, int grp, int trow, size_t block, size_t nblocks,
-                             float* acc) {
+                             const float* pivot, float* acc) {
   constexpr int V = Vec<T>::N;
   using Raw = typename Vec<T>::Raw;
   const size_t step = nblocks * (size_t)rpb;
@@ -301,18 +311,21 @@ BNET_HD void bn_stats_thread(const T* z, size_t rows, int cvec, int rpb, int grp
         Vec<T>::unpack(raw[u], f);
 #pragma unroll
         for (int k = 0; k < V; k++) {
-          acc[k] += f[k];
-          acc[V + k] += f[k] * f[k];
+          const float d = f[k] - pivot[k];
+          acc[k] += d;
+          acc[V + k] += d * d;
         }
       }
     }
   }
 }
 
-// y = relu?( z * scale + shift (+ res) ) with per-channel scale/shift held by the thread
+// y = relu?( (z - mean) * scale + beta (+ res) ) with per-channel mean, scale = gamma * invstd and beta held by the thread.
+// (z * scale + (beta - mean * scale) would save a subtraction but round z * scale, an error of 2^-24 |mean| * scale: far more
+//  than the result's own rounding once |mean| is large next to std, and y = beta would not hold on a constant channel.)
 template <typename T, int U>
 BNET_HD void bn_apply_thread(const T* z, const T* res, T* y, size_t rows, int cvec, int rpb, int grp, int trow, size_t block,
-                             size_t nblocks, const float* scale, const float* shift, bool relu) {
+                             size_t nblocks, const float* mean, const float* scale, const float* beta, bool relu) {
   constexpr int V = Vec<T>::N;
   using Raw = typename Vec<T>::Raw;
   const size_t step = nblocks * (size_t)rpb;
@@ -334,7 +347,7 @@ BNET_HD void bn_apply_thread(const T* z, const T* res, T* y, size_t rows, int cv
         if (res) Vec<T>::unpack(rr[u], q);
 #pragma unroll
         for (int k = 0; k < V; k++) {
-          float v = f[k] * scale[k] + shift[k];
+          float v = (f[k] - mean[k]) * scale[k] + beta[k];
           if (res) v += q[k];
           f[k] = relu ? bnet::nn::relu(v) : v;
         }

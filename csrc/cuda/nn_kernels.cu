@@ -121,14 +121,15 @@ template <typename T>
 __global__ void __launch_bounds__(256) bn_stats_kernel(const T* __restrict__ z, float* __restrict__ stats, size_t rows, int cvec) {
   constexpr int V = Vec<T>::N;
   extern __shared__ float smem[];
-  float acc[2 * V];
+  float acc[2 * V], pivot[V];
 #pragma unroll
   for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
-  bn_stats_thread<T, 4>(z, rows, cvec, blockDim.x / cvec, threadIdx.x % cvec, threadIdx.x / cvec, blockIdx.x, gridDim.x, acc);
+  bn_pivot<T>(z, threadIdx.x % cvec, pivot);
+  bn_stats_thread<T, 4>(z, rows, cvec, blockDim.x / cvec, threadIdx.x % cvec, threadIdx.x / cvec, blockIdx.x, gridDim.x, pivot, acc);
   const int C = cvec * V;
-  reduce_bias_grad<V>(acc, stats, 2 * C, cvec, smem);          // sum
+  reduce_bias_grad<V>(acc, stats, 2 * C, cvec, smem);          // sum of z - pivot
   __syncthreads();
-  reduce_bias_grad<V>(acc + V, stats + C, 2 * C, cvec, smem);  // sum of squares
+  reduce_bias_grad<V>(acc + V, stats + C, 2 * C, cvec, smem);  // sum of (z - pivot)^2
 }
 
 // y = relu?(bn(z) (+ res)); block 0 also updates the running statistics (unbiased variance, PyTorch semantics)
@@ -140,13 +141,14 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ z, 
                                                        float momentum, int relu) {
   constexpr int V = Vec<T>::N;
   const int C = cvec * V, grp = threadIdx.x % cvec, trow = threadIdx.x / cvec;
-  float mean[V], invstd[V], var[V], scale[V], shift[V];
-  bn_moments<V>(stats, C, grp, 1.0f / (float)rows, eps, mean, invstd, var);
+  float pivot[V], mean[V], invstd[V], var[V], scale[V], bet[V];
+  bn_pivot<T>(z, grp, pivot);
+  bn_moments<V>(stats, pivot, C, grp, 1.0f / (float)rows, eps, mean, invstd, var);
 #pragma unroll
   for (int k = 0; k < V; k++) {
     const int c = grp * V + k;
     scale[k] = to_f<T>(gamma[c]) * invstd[k];
-    shift[k] = to_f<T>(beta[c]) - mean[k] * scale[k];
+    bet[k] = to_f<T>(beta[c]);
   }
   if (blockIdx.x == 0 && trow == 0 && running_mean) {
     const float unbias = rows > 1 ? (float)rows / (float)(rows - 1) : 1.0f;
@@ -157,7 +159,7 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ z, 
       running_var[c] = from_f<T>((1.f - momentum) * to_f<T>(running_var[c]) + momentum * var[k] * unbias);
     }
   }
-  bn_apply_thread<T, 4>(z, res, y, rows, cvec, blockDim.x / cvec, grp, trow, blockIdx.x, gridDim.x, scale, shift, relu != 0);
+  bn_apply_thread<T, 4>(z, res, y, rows, cvec, blockDim.x / cvec, grp, trow, blockIdx.x, gridDim.x, mean, scale, bet, relu != 0);
 }
 
 template <typename T>
@@ -167,8 +169,9 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const T* __restrict_
   constexpr int V = Vec<T>::N;
   extern __shared__ float smem[];
   const int C = cvec * V, grp = threadIdx.x % cvec, trow = threadIdx.x / cvec;
-  float mean[V], invstd[V], var[V], acc[2 * V];
-  bn_moments<V>(stats, C, grp, 1.0f / (float)rows, eps, mean, invstd, var);
+  float pivot[V], mean[V], invstd[V], var[V], acc[2 * V];
+  bn_pivot<T>(z, grp, pivot);
+  bn_moments<V>(stats, pivot, C, grp, 1.0f / (float)rows, eps, mean, invstd, var);
 #pragma unroll
   for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
   bn_bwd_reduce_thread<T, 2>(gy, y, z, rows, cvec, blockDim.x / cvec, grp, trow, blockIdx.x, gridDim.x, mean, invstd, relu != 0, acc);
@@ -187,8 +190,9 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__
   constexpr int V = Vec<T>::N;
   const int C = cvec * V, grp = threadIdx.x % cvec, trow = threadIdx.x / cvec;
   const float inv_m = 1.0f / (float)rows;
-  float mean[V], invstd[V], var[V], a[V], c1[V], c2[V];
-  bn_moments<V>(stats, C, grp, inv_m, eps, mean, invstd, var);
+  float pivot[V], mean[V], invstd[V], var[V], a[V], c1[V], c2[V];
+  bn_pivot<T>(z, grp, pivot);
+  bn_moments<V>(stats, pivot, C, grp, inv_m, eps, mean, invstd, var);
 #pragma unroll
   for (int k = 0; k < V; k++) {
     const int c = grp * V + k;
@@ -322,8 +326,9 @@ BNET_API int bnet_nn_pool_relu_bwd_bias_grad(const void* gp, const void* idx, vo
 }
 
 
-// ---- BatchNorm family.  stats / gsum: 2*C floats ([sum | sumsq], [s1 | s2]) that the caller zeroes before the
-// reduce kernels.  gamma/beta/running stats have the activation dtype.  res, running_*, gres may be NULL.
+// ---- BatchNorm family.  stats / gsum: 2*C floats ([sum | sumsq] of z - K, [s1 | s2]) that the caller zeroes before the
+// reduce kernels; K is each channel's value in row 0 of z (nn_body.cuh, bn_moments), which the kernels that read stats
+// load from z themselves.  gamma/beta/running stats have the activation dtype.  res, running_*, gres may be NULL.
 namespace {
 struct RowGrid { int threads, grid; size_t smem; };
 RowGrid row_grid(long long rows, int cvec, int V, int accs) {

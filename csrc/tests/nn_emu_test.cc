@@ -202,27 +202,30 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
     gamma[c] = Conv<T>::to(0.5f + 0.01f * (c % 37));
     beta[c] = Conv<T>::to(-0.3f + 0.02f * (c % 11));
   }
-  // ---- statistics
+  // ---- statistics: sums of z - K and (z - K)^2, K = the channel's value in row 0
   std::vector<double> st(2 * C, 0.0);
   for (int b = 0; b < nblocks; b++)
     for (int t = 0; t < threads; t++) {
-      float acc[2 * V];
+      float acc[2 * V], piv[V];
       for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
-      bn_stats_thread<T, 4>(z.data(), rows, cvec, rpb, t % cvec, t / cvec, (size_t)b, (size_t)nblocks, acc);
+      bn_pivot<T>(z.data(), t % cvec, piv);
+      bn_stats_thread<T, 4>(z.data(), rows, cvec, rpb, t % cvec, t / cvec, (size_t)b, (size_t)nblocks, piv, acc);
       for (int k = 0; k < V; k++) {
         st[(t % cvec) * V + k] += acc[k];
         st[C + (t % cvec) * V + k] += acc[V + k];
       }
     }
-  std::vector<double> rsum(C, 0.0), rsq(C, 0.0);
+  std::vector<double> rsum(C, 0.0), rsq(C, 0.0), dsum(C, 0.0), dsq(C, 0.0);
   for (size_t i = 0; i < rows * C; i++) {
-    double v = Conv<T>::from(z[i]);
+    double v = Conv<T>::from(z[i]), d = v - Conv<T>::from(z[i % C]);
     rsum[i % C] += v;
     rsq[i % C] += v * v;
+    dsum[i % C] += d;
+    dsq[i % C] += d * d;
   }
   for (int c = 0; c < C; c++) {
-    CHECK(fabs(st[c] - rsum[c]) <= 1e-3 * (1.0 + fabs(rsum[c])), "%s bn sum c=%d %f vs %f", Conv<T>::name(), c, st[c], rsum[c]);
-    CHECK(fabs(st[C + c] - rsq[c]) <= 1e-3 * (1.0 + fabs(rsq[c])), "%s bn sumsq c=%d", Conv<T>::name(), c);
+    CHECK(fabs(st[c] - dsum[c]) <= 1e-3 * (1.0 + fabs(dsum[c])), "%s bn sum c=%d %f vs %f", Conv<T>::name(), c, st[c], dsum[c]);
+    CHECK(fabs(st[C + c] - dsq[c]) <= 1e-3 * (1.0 + fabs(dsq[c])), "%s bn sumsq c=%d", Conv<T>::name(), c);
   }
   std::vector<float> stats(2 * C);
   for (int i = 0; i < 2 * C; i++) stats[i] = (float)st[i];
@@ -232,14 +235,15 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
   for (int b = 0; b < nblocks; b++)
     for (int t = 0; t < threads; t++) {
       const int grp = t % cvec;
-      float mean[V], invstd[V], var[V], scale[V], shift[V];
-      bn_moments<V>(stats.data(), C, grp, inv_m, eps, mean, invstd, var);
+      float piv[V], mean[V], invstd[V], var[V], scale[V], shift[V];
+      bn_pivot<T>(z.data(), grp, piv);
+      bn_moments<V>(stats.data(), piv, C, grp, inv_m, eps, mean, invstd, var);
       for (int k = 0; k < V; k++) {
         scale[k] = Conv<T>::from(gamma[grp * V + k]) * invstd[k];
-        shift[k] = Conv<T>::from(beta[grp * V + k]) - mean[k] * scale[k];
+        shift[k] = Conv<T>::from(beta[grp * V + k]);
       }
       bn_apply_thread<T, 4>(z.data(), with_res ? res.data() : nullptr, y.data(), rows, cvec, rpb, grp, t / cvec, (size_t)b,
-                            (size_t)nblocks, scale, shift, relu);
+                            (size_t)nblocks, mean, scale, shift, relu);
     }
   std::vector<double> mean(C), invstd(C);
   for (int c = 0; c < C; c++) {
@@ -261,8 +265,9 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
   for (int b = 0; b < nblocks; b++)
     for (int t = 0; t < threads; t++) {
       const int grp = t % cvec;
-      float mn[V], is[V], var[V], acc[2 * V];
-      bn_moments<V>(stats.data(), C, grp, inv_m, eps, mn, is, var);
+      float piv[V], mn[V], is[V], var[V], acc[2 * V];
+      bn_pivot<T>(z.data(), grp, piv);
+      bn_moments<V>(stats.data(), piv, C, grp, inv_m, eps, mn, is, var);
       for (int k = 0; k < 2 * V; k++) acc[k] = 0.f;
       bn_bwd_reduce_thread<T, 2>(gy.data(), y.data(), z.data(), rows, cvec, rpb, grp, t / cvec, (size_t)b, (size_t)nblocks, mn, is, relu, acc);
       for (int k = 0; k < V; k++) {
@@ -287,8 +292,9 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
   for (int b = 0; b < nblocks; b++)
     for (int t = 0; t < threads; t++) {
       const int grp = t % cvec;
-      float mn[V], is[V], var[V], a[V], c1[V], c2[V];
-      bn_moments<V>(stats.data(), C, grp, inv_m, eps, mn, is, var);
+      float piv[V], mn[V], is[V], var[V], a[V], c1[V], c2[V];
+      bn_pivot<T>(z.data(), grp, piv);
+      bn_moments<V>(stats.data(), piv, C, grp, inv_m, eps, mn, is, var);
       for (int k = 0; k < V; k++) {
         a[k] = Conv<T>::from(gamma[grp * V + k]) * is[k];
         c1[k] = gsum[grp * V + k] * inv_m;
@@ -309,7 +315,7 @@ static void test_bn(size_t rows, int C, int nblocks, bool relu, bool with_res) {
   }
 }
 
-// BatchNorm apply / backward with ReLU on activations holding NaN and +-Inf: scale 1, shift 0 makes y = relu(z), and the
+// BatchNorm apply / backward with ReLU on activations holding NaN and +-Inf: mean 0, scale 1, beta 0 make y = relu(z), and the
 // backward passes dy wherever torch's threshold_backward would (y NaN included)
 template <typename T>
 static void test_bn_specials(size_t rows, int C) {
@@ -322,7 +328,7 @@ static void test_bn_specials(size_t rows, int C) {
   for (int k = 0; k < V; k++) { one[k] = 1.f; zero[k] = 0.f; }
   memset((void*)y.data(), 0x7f, y.size() * sizeof(T));
   for (int t = 0; t < threads; t++)
-    bn_apply_thread<T, 4>(z.data(), nullptr, y.data(), rows, cvec, rpb, t % cvec, t / cvec, 0, 1, one, zero, true);
+    bn_apply_thread<T, 4>(z.data(), nullptr, y.data(), rows, cvec, rpb, t % cvec, t / cvec, 0, 1, zero, one, zero, true);
   for (size_t i = 0; i < rows * C; i++)
     CHECK(same_or_nan(y[i], Conv<T>::to(relu_ref(Conv<T>::from(z[i])))), "%s bn apply relu i=%zu", Conv<T>::name(), i);
   // mean 0, invstd 1, a 1, c1 = c2 = 0: gz = dy - z * 0, and gres = dy
@@ -344,6 +350,124 @@ static void test_bn_specials(size_t rows, int C) {
     CHECK(same_or_nan(gz[i], Conv<T>::to(want)), "%s bn bwd gz i=%zu", Conv<T>::name(), i);
   }
   for (int c = 0; c < C; c++) CHECK(close_sum(s1[c], r1[c]), "%s bn bwd s1 c=%d", Conv<T>::name(), c);
+}
+
+// bn_stats as the GPU adds it up, in the kernels' float order: each thread's walk, the block's rows of threads in ascending
+// order (reduce_bias_grad), then the blocks' partial rows b = g (mod 8) per g and the 8 sums in order (sum_rows_kernel)
+template <typename T>
+static std::vector<float> emu_bn_stats(const std::vector<T>& z, size_t rows, int C, int nblocks) {
+  constexpr int V = Vec<T>::N;
+  const int cvec = C / V, threads = (256 / cvec) * cvec, rpb = threads / cvec;
+  std::vector<float> part((size_t)nblocks * 2 * C, 0.f);
+  std::vector<float> acc((size_t)threads * 2 * V);
+  for (int b = 0; b < nblocks; b++) {
+    for (int t = 0; t < threads; t++) {
+      float* a = &acc[(size_t)t * 2 * V];
+      float piv[V];
+      for (int k = 0; k < 2 * V; k++) a[k] = 0.f;
+      bn_pivot<T>(z.data(), t % cvec, piv);
+      bn_stats_thread<T, 4>(z.data(), rows, cvec, rpb, t % cvec, t / cvec, (size_t)b, (size_t)nblocks, piv, a);
+    }
+    for (int g = 0; g < cvec; g++)
+      for (int k = 0; k < 2 * V; k++) {
+        float s = 0.f;
+        for (int r = 0; r < rpb; r++) s += acc[(size_t)(r * cvec + g) * 2 * V + k];
+        part[(size_t)b * 2 * C + (k < V ? 0 : C) + g * V + k % V] = s;
+      }
+  }
+  std::vector<float> stats(2 * C);
+  for (int c = 0; c < 2 * C; c++) {
+    float sums[8];
+    for (int g = 0; g < 8; g++) {
+      sums[g] = 0.f;
+      for (int b = g; b < nblocks; b += 8) sums[g] += part[(size_t)b * 2 * C + c];
+    }
+    float t = sums[0];
+    for (int g = 1; g < 8; g++) t += sums[g];
+    stats[c] = 0.f + t;
+  }
+  return stats;
+}
+
+// BatchNorm statistics of channels far from zero: channel c holds off[c] + sd * N(0, 1), and mean / std reaches 2^10.  The
+// variance must stay within 2^-16 of a two-pass float64 variance of the same values, the mean within
+// 2^-22 |mean| + 2^-20 std; a constant channel has variance 0 exactly.  Plain sums of z and z^2 lose (mean / std)^2 * 2^-24.
+// bf16: channels made of three adjacent bf16 values around 2^e (mean / std near 2^7).
+template <typename T>
+static void test_bn_offset(size_t rows, int C, int nblocks) {
+  constexpr int V = Vec<T>::N;
+  const bool bf = sizeof(T) == 2;
+  const double ratios[] = {0, 4, 16, 64, 256, 1024};
+  const int nr = bf ? 1 : 6;
+  std::vector<T> z(rows * C);
+  std::vector<double> sd(C);
+  unsigned s = 777u + (unsigned)C;
+  auto gauss = [&]() {   // sum of 4 uniforms, scaled to unit variance
+    double a = 0;
+    for (int i = 0; i < 4; i++) { s = s * 1664525u + 1013904223u; a += ((s >> 8) & 0xffff) / 65536.0 - 0.5; }
+    return a * sqrt(3.0);
+  };
+  for (int c = 0; c < C; c++) sd[c] = ldexp(1.0, (c % 7) - 3);
+  for (size_t i = 0; i < rows * C; i++) {
+    const int c = (int)(i % C);
+    double v;
+    if (c == C - 1) v = 3.0 * sd[c];                                       // a constant channel
+    else if (bf) v = ldexp(1.0 + ((s = s * 1664525u + 1013904223u) >> 16) % 3 / 128.0, (c % 9) - 4);
+    else v = ratios[c % nr] * sd[c] + sd[c] * gauss();
+    z[i] = Conv<T>::to((float)v);
+  }
+  const std::vector<float> stats = emu_bn_stats<T>(z, rows, C, nblocks);
+  const float inv_m = 1.0f / (float)rows;
+  double worst = 0;
+  for (int grp = 0; grp < C / V; grp++) {
+    float piv[V], mean[V], invstd[V], var[V];
+    bn_pivot<T>(z.data(), grp, piv);
+    bn_moments<V>(stats.data(), piv, C, grp, inv_m, 1e-5f, mean, invstd, var);
+    for (int k = 0; k < V; k++) {
+      const int c = grp * V + k;
+      double m = 0, v = 0;
+      for (size_t r = 0; r < rows; r++) m += Conv<T>::from(z[r * C + c]);
+      m /= rows;
+      for (size_t r = 0; r < rows; r++) { const double d = Conv<T>::from(z[r * C + c]) - m; v += d * d; }
+      v /= rows;
+      const double bv = ldexp(v, -16), bm = ldexp(fabs(m), -22) + ldexp(sqrt(v), -20);
+      CHECK(fabs(var[k] - v) <= bv, "%s bn offset var rows=%zu C=%d c=%d mean/std=%.0f: %.9g vs %.9g (rel %.2e)", Conv<T>::name(), rows, C, c,
+            fabs(m) / sqrt(v), var[k], v, fabs(var[k] - v) / v);
+      CHECK(fabs(mean[k] - m) <= bm, "%s bn offset mean rows=%zu C=%d c=%d: %.9g vs %.9g", Conv<T>::name(), rows, C, c, mean[k], m);
+      if (v == 0) CHECK(var[k] == 0.f && (double)mean[k] == m, "%s bn constant channel c=%d: var %g mean %g", Conv<T>::name(), c, var[k], mean[k]);
+      if (v > 0) worst = fmax(worst, fabs(var[k] - v) / bv);
+    }
+  }
+  printf("  %s bn statistics of offset channels, rows=%zu C=%d blocks=%d: worst var error / 2^-16 var = %.3f\n", Conv<T>::name(), rows, C,
+         nblocks, worst);
+}
+
+// an Inf or a NaN in a channel (in row 0, the pivot, or further down) makes its variance NaN, as in eager torch; the other
+// channels keep their statistics
+template <typename T>
+static void test_bn_stats_nonfinite(size_t rows, int C, int nblocks) {
+  constexpr int V = Vec<T>::N;
+  std::vector<T> z(rows * C);
+  for (auto& v : z) v = Conv<T>::to(frand());
+  const float bad[3] = {INFINITY, -INFINITY, NAN};
+  // channel 3j+q gets bad[q] in row 0 (j = 0) or in row 5 + j (j > 0)
+  const int nbad = C < 9 ? C : 9;
+  for (int c = 0; c < nbad; c++) z[(c < 3 ? 0 : (size_t)(5 + c / 3) % rows) * C + c] = Conv<T>::to(bad[c % 3]);
+  const std::vector<float> stats = emu_bn_stats<T>(z, rows, C, nblocks);
+  for (int grp = 0; grp < C / V; grp++) {
+    float piv[V], mean[V], invstd[V], var[V];
+    bn_pivot<T>(z.data(), grp, piv);
+    bn_moments<V>(stats.data(), piv, C, grp, 1.0f / (float)rows, 1e-5f, mean, invstd, var);
+    for (int k = 0; k < V; k++) {
+      const int c = grp * V + k;
+      if (c < nbad)
+        CHECK(var[k] != var[k] && invstd[k] != invstd[k], "%s bn stats: channel %d holds %g, var %g invstd %g (want NaN)", Conv<T>::name(), c,
+              bad[c % 3], var[k], invstd[k]);
+      else
+        CHECK(var[k] == var[k] && var[k] > 0.f && mean[k] == mean[k], "%s bn stats: finite channel %d has var %g mean %g", Conv<T>::name(), c,
+              var[k], mean[k]);
+    }
+  }
 }
 
 template <typename T>
@@ -393,11 +517,33 @@ static void run_specials() {
   test_bn_specials<T>(100, 8 * V);
 }
 
+// the reduce kernels' grid (row_grid in nn_kernels.cu) with the planner's 132 SMs and 2 blocks per SM
+static int bn_grid(size_t rows, int C, int V) {
+  const int cvec = C / V, rpb = ((256 / cvec) * cvec) / cvec;
+  const size_t want = (rows + 8 * (size_t)rpb - 1) / (8 * (size_t)rpb);
+  return want < 264 ? (int)want : 264;
+}
+
+// BatchNorm statistics at ResNet-50 shapes with channels far from zero, and non-finite values through the statistics
+template <typename T>
+static void run_bn_statistics() {
+  constexpr int V = Vec<T>::N;
+  const size_t layer1 = 8 * 56 * 56, stem = 32 * 112 * 112;
+  test_bn_offset<T>(layer1, 64, bn_grid(layer1, 64, V));
+  test_bn_offset<T>(stem, 64, bn_grid(stem, 64, V));
+  test_bn_offset<T>(2 * 7 * 7, 256 * V, bn_grid(2 * 7 * 7, 256 * V, V));
+  test_bn_offset<T>(2, 8 * V, 1);
+  test_bn_stats_nonfinite<T>(257, 8 * V, 3);
+  test_bn_stats_nonfinite<T>(layer1, 64, bn_grid(layer1, 64, V));
+}
+
 int main() {
   run_all<float>();
   run_all<__nv_bfloat16>();
   run_specials<float>();
   run_specials<__nv_bfloat16>();
+  run_bn_statistics<float>();
+  run_bn_statistics<__nv_bfloat16>();
   printf("%s (%d failure%s)\n", g_fail ? "FAILED" : "nn kernel emulation tests passed", g_fail, g_fail == 1 ? "" : "s");
   return g_fail ? 1 : 0;
 }

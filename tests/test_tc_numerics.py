@@ -52,5 +52,7 @@ def test_nan_and_inf_follow_eager_torch():
 
 
 @pytest.mark.gpu
-def test_fused_column_reductions_are_reproducible():
+def test_fused_column_reductions_are_reproducible_with_shifted_bn_stats():
+    """Bias-gradient and BatchNorm reductions give identical bits in three calls; the BatchNorm statistics are the sums of
+    z - K and (z - K)^2 with K each channel's row-0 value."""
     _job("reductions")
