@@ -86,24 +86,31 @@ $(BUILD)/tests/exec_emu_test: csrc/tests/exec_emu_test.cc csrc/cuda/exec_body.cu
 $(BUILD)/tests/tc_emu_test: csrc/tests/tc_emu_test.cc csrc/cuda/tc_body.cuh include/bnet/bnet_tc.h
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) -Iinclude $< -o $@
+# the fused AdamW kernel's per-element update against a long-double AdamW
+$(BUILD)/tests/optim_emu_test: csrc/tests/optim_emu_test.cc csrc/cuda/optim_body.cuh
+	@mkdir -p $(dir $@)
+	$(CXX) $(EMU_FLAGS) $< -o $@
 
 # the same emulation tests under Address/UB sanitizers: an out-of-bounds or misaligned access of a kernel body
 # is caught here, on the CPU, instead of poisoning a CUDA context
-emu-asan: csrc/tests/nn_emu_test.cc csrc/tests/exec_emu_test.cc csrc/tests/tc_emu_test.cc csrc/cuda/nn_body.cuh csrc/cuda/exec_body.cuh csrc/cuda/tc_body.cuh
+emu-asan: csrc/tests/nn_emu_test.cc csrc/tests/exec_emu_test.cc csrc/tests/tc_emu_test.cc csrc/tests/optim_emu_test.cc csrc/cuda/nn_body.cuh csrc/cuda/exec_body.cuh csrc/cuda/tc_body.cuh csrc/cuda/optim_body.cuh
 	@mkdir -p $(BUILD)/asan/tests
 	$(SAN_CXX) $(EMU_FLAGS) -O1 -w $(SAN_FLAGS_asan) csrc/tests/nn_emu_test.cc -o $(BUILD)/asan/tests/nn_emu_test
 	$(SAN_CXX) $(EMU_FLAGS) -O1 -w $(SAN_FLAGS_asan) csrc/tests/exec_emu_test.cc -o $(BUILD)/asan/tests/exec_emu_test
 	$(SAN_CXX) $(EMU_FLAGS) -Iinclude -O1 -w $(SAN_FLAGS_asan) csrc/tests/tc_emu_test.cc -o $(BUILD)/asan/tests/tc_emu_test
+	$(SAN_CXX) $(EMU_FLAGS) -O1 -w $(SAN_FLAGS_asan) csrc/tests/optim_emu_test.cc -o $(BUILD)/asan/tests/optim_emu_test
 	$(BUILD)/asan/tests/nn_emu_test
 	$(BUILD)/asan/tests/exec_emu_test
 	$(BUILD)/asan/tests/tc_emu_test
+	$(BUILD)/asan/tests/optim_emu_test
 
-test: $(TEST_BINS) $(BUILD)/tests/nn_emu_test $(BUILD)/tests/exec_emu_test $(BUILD)/tests/tc_emu_test
+test: $(TEST_BINS) $(BUILD)/tests/nn_emu_test $(BUILD)/tests/exec_emu_test $(BUILD)/tests/tc_emu_test $(BUILD)/tests/optim_emu_test
 	$(BUILD)/tests/unit_tests $(PLUGIN_SO)
 	$(BUILD)/tests/loopback_test $(PLUGIN_SO)
 	$(BUILD)/tests/nn_emu_test
 	$(BUILD)/tests/exec_emu_test
 	$(BUILD)/tests/tc_emu_test
+	$(BUILD)/tests/optim_emu_test
 
 BENCH_BINS := $(BUILD)/bench/all_reduce_perf
 NCCL_HOME ?= $(shell python -c "import nvidia.nccl, os; print(os.path.dirname(nvidia.nccl.__file__))" 2>/dev/null)

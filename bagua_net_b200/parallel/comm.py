@@ -77,6 +77,7 @@ def _declare(lib):
     lib.bnet_fused_allreduce_sgd.argtypes = [vp, sz, sz, sz, i, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp,
                                              i, i, i, vp]
     lib.bnet_fused_allreduce_sgd_hp.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, i, i, i, vp]
+    lib.bnet_fused_allreduce_adamw.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, vp, i, i, i, vp]
     lib.bnet_pack_cast.argtypes = [vp, i, vp, i, i, C.c_float, C.c_uint64, vp]
 
 
@@ -256,6 +257,23 @@ class SymmComm:
             self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], lr, momentum,
             weight_decay, gs, C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), 1 if zero_grads else 0,
             channel, nblocks, self._stream(stream)), "fused_allreduce_sgd")
+        self.launches += n
+
+    def fused_allreduce_adamw(self, grad: torch.Tensor, param: torch.Tensor, master: torch.Tensor, exp_avg: torch.Tensor,
+                              exp_avg_sq: torch.Tensor, hp: torch.Tensor, zero_grads: bool = True, channel: int = 0,
+                              nblocks: int = 0, stream=None):
+        """One kernel: sum-reduce ``grad`` across ranks, AdamW-update this rank's fp32 shard (``master`` / ``exp_avg`` /
+        ``exp_avg_sq``: numel/world each) and write the new ``param`` on every rank.  ``hp``: fp32 CUDA tensor of 8
+        elements {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved} that the kernel reads when it runs;
+        ``step`` counts the steps already taken and is not advanced here (the caller does that once per step)."""
+        assert grad.numel() == param.numel() and grad.dtype == param.dtype
+        assert master.dtype == exp_avg.dtype == exp_avg_sq.dtype == torch.float32
+        assert master.numel() * self.world == grad.numel() == exp_avg.numel() * self.world == exp_avg_sq.numel() * self.world
+        assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= 8 and hp.is_contiguous()
+        n = self._chk(self.lib.bnet_fused_allreduce_adamw(
+            self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], C.c_void_p(hp.data_ptr()),
+            C.c_void_p(master.data_ptr()), C.c_void_p(exp_avg.data_ptr()), C.c_void_p(exp_avg_sq.data_ptr()),
+            1 if zero_grads else 0, channel, nblocks, self._stream(stream)), "fused_allreduce_adamw")
         self.launches += n
 
 

@@ -8,7 +8,7 @@ NVSwitch box:
   gradient has a slice of the flat gradient buffer that its producer writes directly (``ops/grad_target.py``) or
   that a hook copies it into — autograd never accumulates (no add pass, no bucket copy-in/copy-out);
 * when the last gradient of a bucket has been produced, ONE kernel on a side stream
-  reduces the bucket in the switch (NVLS), applies SGD+momentum+weight-decay on the owning
+  reduces the bucket in the switch (NVLS), applies the optimizer (SGD+momentum+weight-decay, or AdamW) on the owning
   rank's fp32 master shard, writes the new bf16 parameters to every rank and re-zeroes the
   gradients — overlapping the rest of the backward pass;
 * optimizer state is sharded 1/world (ZeRO-1 style) for free.
@@ -133,7 +133,7 @@ def direct_grads_self_check(device=None, group=None, steps: int = 3, make_model=
 
 
 class _Bucket:
-    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "master", "mom")
+    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "master", "mom", "exp_avg", "exp_avg_sq")
 
     def __init__(self):
         self.params = []
@@ -143,15 +143,32 @@ class _Bucket:
 
 
 class BnetDDP(torch.nn.Module):
-    """Wraps ``module``; owns the optimizer (SGD with momentum, fused into the collective).
+    """Wraps ``module``; owns the optimizer, fused into the collective: ``optimizer="sgd"`` (SGD with momentum and L2
+    weight decay) or ``"adamw"`` (``torch.optim.AdamW`` with ``betas``, ``eps`` and decoupled ``weight_decay``;
+    AMSGrad and ``maximize`` are not offered).
 
     bucket_mb sizes buckets for launch latency and overlap (NVSwitch: no per-link bound).
     """
 
-    def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float = 0.9, weight_decay: float = 0.0,
+    def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float | None = None, weight_decay: float = 0.0,
                  bucket_mb: float = 64.0, comm: SymmComm | None = None, extra_heap_bytes: int = 64 << 20,
-                 nblocks: int = 0, group=None):
+                 nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
+                 eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False):
         super().__init__()
+        if optimizer not in ("sgd", "adamw"):
+            raise ValueError(f"unknown optimizer {optimizer!r}: BnetDDP fuses 'sgd' or 'adamw'")
+        if amsgrad or maximize:
+            raise ValueError("the fused AdamW offers neither amsgrad nor maximize")
+        if optimizer == "adamw":
+            if momentum is not None:
+                raise ValueError("AdamW has no momentum argument; use betas")
+            betas = (float(betas[0]), float(betas[1]))
+            if not (0.0 <= betas[0] < 1.0 and 0.0 <= betas[1] < 1.0) or not eps >= 0.0:
+                raise ValueError(f"AdamW needs 0 <= beta < 1 and eps >= 0 (got betas={betas}, eps={eps})")
+            self.betas, self.eps = betas, float(eps)
+        elif momentum is None:
+            momentum = 0.9
+        self.optimizer = optimizer
         self.module = module
         self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
         self.nblocks = nblocks
@@ -237,13 +254,20 @@ class BnetDDP(torch.nn.Module):
             dist.barrier(group=group)
             comm.all_reduce(self.flat_param, "sum")
             torch.cuda.synchronize()
-        # fp32 master weights + momentum for this rank's shard of every bucket
+        # fp32 master weights + optimizer state (momentum, or AdamW's two moments) for this rank's shard of every bucket
         for b in self.buckets:
             b.grad = self.flat_grad[b.start:b.start + b.numel]
             b.param = self.flat_param[b.start:b.start + b.numel]
             shard = b.numel // comm.world
             b.master = b.param[comm.rank * shard:(comm.rank + 1) * shard].float().contiguous()
-            b.mom = torch.zeros_like(b.master)
+            if optimizer == "adamw":
+                b.exp_avg = torch.zeros_like(b.master)
+                b.exp_avg_sq = torch.zeros_like(b.master)
+            else:
+                b.mom = torch.zeros_like(b.master)
+        if optimizer == "adamw":
+            # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh)
+            self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev)
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad) for p in params]
@@ -272,9 +296,13 @@ class BnetDDP(torch.nn.Module):
         ev = torch.cuda.Event()
         ev.record(cur)
         self.comm_stream.wait_event(ev)          # the bucket's gradients are complete on the compute stream
-        self.comm.fused_allreduce_sgd(b.grad, b.param, b.master, b.mom, self.lr, self.momentum, self.weight_decay,
-                                      zero_grads=True, channel=0, nblocks=self.nblocks, stream=self.comm_stream,
-                                      hp=getattr(self, "_hp", None))
+        if self.optimizer == "adamw":
+            self.comm.fused_allreduce_adamw(b.grad, b.param, b.master, b.exp_avg, b.exp_avg_sq, self._hp, zero_grads=True,
+                                            channel=0, nblocks=self.nblocks, stream=self.comm_stream)
+        else:
+            self.comm.fused_allreduce_sgd(b.grad, b.param, b.master, b.mom, self.lr, self.momentum, self.weight_decay,
+                                          zero_grads=True, channel=0, nblocks=self.nblocks, stream=self.comm_stream,
+                                          hp=getattr(self, "_hp", None))
         b.ready = 0
         self._inflight = True
 
@@ -284,6 +312,11 @@ class BnetDDP(torch.nn.Module):
             if b.ready:                           # parameters that got no gradient this step
                 self._launch(b)
         if self._inflight:
+            if self.optimizer == "adamw":
+                # one optimizer step taken: advance the step count the kernels read, behind this step's last bucket
+                # (on the comm stream, so a captured step replays it)
+                with torch.cuda.stream(self.comm_stream):
+                    self._hp[self._HP_STEP:self._HP_STEP + 1].add_(1.0)
             torch.cuda.current_stream().wait_stream(self.comm_stream)
             self._inflight = False
 
@@ -320,7 +353,9 @@ class BnetDDP(torch.nn.Module):
             # master weights, momentum, module buffers (BatchNorm running statistics).  A (re)capture therefore
             # leaves the training trajectory exactly where eager mode would have it; checkpoint/resume stays
             # step-exact.
-            saved = [self.flat_param.clone()] + [t.clone() for b in self.buckets for t in (b.master, b.mom)]
+            saved = [self.flat_param.clone()] + [t.clone() for b in self.buckets for t in self._state(b)]
+            if self.optimizer == "adamw":
+                saved.append(self._hp.clone())      # (the step count)
             bufs = [t for t in self.module.buffers() if t.is_cuda and t.numel()]
             saved_bufs = [t.clone() for t in bufs]
             for _ in range(2):
@@ -331,8 +366,10 @@ class BnetDDP(torch.nn.Module):
             it = iter(saved)
             self.flat_param.copy_(next(it))
             for b in self.buckets:
-                b.master.copy_(next(it))
-                b.mom.copy_(next(it))
+                for t in self._state(b):
+                    t.copy_(next(it))
+            if self.optimizer == "adamw":
+                self._hp.copy_(next(it))
             for t, s in zip(bufs, saved_bufs):
                 t.copy_(s)
             del saved, saved_bufs
@@ -452,20 +489,38 @@ class BnetDDP(torch.nn.Module):
     # ------------------------------------------------------------------ checkpoint / resume
     # Model weights live in ordinary nn.Module tensors (views into the flat heap), so module.state_dict() /
     # load_state_dict() work unchanged.  The optimizer state is this rank's 1/world shard of the fp32 master
-    # weights and momentum of every bucket.
+    # weights and momentum (SGD) or exp_avg / exp_avg_sq (AdamW, which also saves its step count) of every bucket.
     def optimizer_state_dict(self) -> dict:
+        if self.optimizer == "adamw":
+            return {"optimizer": "adamw", "lr": self.lr, "betas": self.betas, "eps": self.eps,
+                    "weight_decay": self.weight_decay, "step": int(self._hp[self._HP_STEP].item()),
+                    "world": self.comm.world, "rank": self.comm.rank,
+                    "buckets": [{"master": b.master.detach().cpu(), "exp_avg": b.exp_avg.detach().cpu(),
+                                 "exp_avg_sq": b.exp_avg_sq.detach().cpu()} for b in self.buckets]}
         return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay,
                 "world": self.comm.world, "rank": self.comm.rank,
                 "buckets": [{"master": b.master.detach().cpu(), "momentum": b.mom.detach().cpu()} for b in self.buckets]}
 
     def load_optimizer_state_dict(self, state: dict) -> None:
+        kind = state.get("optimizer", "sgd")
+        if kind != self.optimizer:
+            raise ValueError(f"optimizer state of {kind!r} cannot be loaded into a {self.optimizer!r} engine")
         if state["world"] != self.comm.world or state["rank"] != self.comm.rank or len(state["buckets"]) != len(self.buckets):
             raise ValueError("optimizer state was saved for a different world size / rank / bucket layout")
         for b, s in zip(self.buckets, state["buckets"]):
             if s["master"].shape != b.master.shape:
                 raise ValueError("optimizer state shard does not match this bucket")
             b.master.copy_(s["master"])
-            b.mom.copy_(s["momentum"])
+            if self.optimizer == "adamw":
+                b.exp_avg.copy_(s["exp_avg"])
+                b.exp_avg_sq.copy_(s["exp_avg_sq"])
+            else:
+                b.mom.copy_(s["momentum"])
+        if self.optimizer == "adamw":
+            self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
+            self.betas = tuple(state["betas"])
+            self._hp.copy_(torch.tensor(self._adamw_hp(state["step"]), dtype=torch.float32))
+            return
         self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
         if getattr(self, "_hp", None) is not None:
             self.set_lr(self.lr)              # hyper-parameters live in device memory: refresh them
@@ -491,7 +546,17 @@ class BnetDDP(torch.nn.Module):
     def set_lr(self, lr: float, momentum: float | None = None, weight_decay: float | None = None):
         """Learning-rate schedule hook.  From the first call on, the fused optimizer kernels read {lr, momentum,
         weight decay, 1/world} from a 4-float device tensor instead of baked-in launch arguments, so a captured CUDA
-        graph is re-captured once (here) and then follows the schedule with one tiny host→device write per change."""
+        graph is re-captured once (here) and then follows the schedule with one tiny host→device write per change.
+        AdamW reads its hyper-parameters from device memory from the start (no re-capture at all) and has no momentum."""
+        if self.optimizer == "adamw":
+            if momentum is not None:
+                raise ValueError("AdamW has no momentum; its betas are fixed at construction")
+            self.lr = float(lr)
+            if weight_decay is not None:
+                self.weight_decay = float(weight_decay)
+            # everything but the step count, which the captured steps advance on the device
+            self._hp[:self._HP_STEP].copy_(torch.tensor(self._adamw_hp(0)[:self._HP_STEP], dtype=torch.float32))
+            return
         self.lr = float(lr)
         if momentum is not None:
             self.momentum = float(momentum)
@@ -503,6 +568,16 @@ class BnetDDP(torch.nn.Module):
             self._graph = None
         else:
             self._hp.copy_(torch.tensor(vals, dtype=torch.float32), non_blocking=False)
+
+    # AdamW's hyper-parameter block: {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved}
+    _HP_STEP = 6
+
+    def _adamw_hp(self, step: int) -> list:
+        return [self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, 1.0 / self.comm.world, float(step), 0.0]
+
+    def _state(self, b: _Bucket) -> tuple:
+        """The fp32 tensors the fused kernel updates for bucket `b`."""
+        return (b.master, b.exp_avg, b.exp_avg_sq) if self.optimizer == "adamw" else (b.master, b.mom)
 
     @property
     def kernel_launches(self) -> int:

@@ -27,6 +27,7 @@
 #include "bnet/bnet_coll.h"
 #include "core/common.h"
 #include "cuda/driver_api.h"
+#include "cuda/optim_body.cuh"
 #include "cuda/ptx.cuh"
 
 #define BNET_API extern "C" __attribute__((visibility("default")))
@@ -422,10 +423,57 @@ __global__ void __launch_bounds__(256) bnet_allreduce_ll_kernel(CollDev d, size_
   }
 }
 
-// ------------------------------------------------------------------ fused all-reduce + SGD + broadcast
+// ------------------------------------------------------------------ fused all-reduce + optimizer + broadcast
 // MODE 0: single GPU, 1: NVLS multicast, 2: peer loads/stores
 //
-// One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch
+// Shared by the SGD and AdamW kernels: the summed gradient vector at heap byte offset `go` (MODE 1: in-switch
+// reduction, raw vector in gv; MODE 2: peer loads summed in fp32 into gf; MODE 0: the local vector in gv) ...
+template <int DT, int MODE>
+__device__ __forceinline__ void fused_grad_issue(const CollDev& d, size_t go, int4& gv, float* gf) {
+  if constexpr (MODE == 1) gv = mc_ld_reduce<DT, BNET_SUM>(d.mc + go);
+  else if constexpr (MODE == 2) p2p_reduce<DT, BNET_SUM>(d, go, d.rank, gf);
+  else gv = ptx::ld_na_v4(reinterpret_cast<const int4*>(d.heap[0] + go));
+}
+template <int DT, int MODE>
+__device__ __forceinline__ void fused_grad_get(const int4& gv, const float* gf, float* g) {
+  if constexpr (MODE == 2) {
+#pragma unroll
+    for (int k = 0; k < VecTraits<DT>::kElems; k++) g[k] = gf[k];
+  } else {
+    unpack<DT>(gv, g);
+  }
+}
+// ... and the new parameter vector `out` stored at heap byte offset `po` on every rank
+template <int MODE>
+__device__ __forceinline__ void fused_param_store(const CollDev& d, size_t po, const int4& out) {
+  if constexpr (MODE == 1) {
+    ptx::multimem_st_v4(d.mc + po, out);          // new parameters land on every rank
+  } else if constexpr (MODE == 2) {
+    for (int j = 0; j < d.world; j++) {
+      int pr = d.rank + j;
+      if (pr >= d.world) pr -= d.world;
+      ptx::st_na_v4(reinterpret_cast<int4*>(d.heap[pr] + po), out);
+    }
+  } else {
+    ptx::st_na_v4(reinterpret_cast<int4*>(d.heap[0] + po), out);
+  }
+}
+
+// Reset our gradients for the next backward, after the closing rank_barrier.  The barrier only pairs CTA b with
+// CTA b of the peers (CTAs of a grid start staggered when the kernel runs under backward on the side stream), so
+// CTA b may only zero what CTA b of some rank has READ: shard p, vectors p*per + i for exactly the i this CTA walks
+// in the update loop.  Zeroing with a flat index would hand vectors of shard p >= 1 to a different CTA than the one
+// rank p reads them with.
+__device__ __forceinline__ void fused_zero_grads(const CollDev& d, size_t goff, size_t nvec, size_t per, size_t stride) {
+  int4* gz = reinterpret_cast<int4*>(d.heap[d.rank] + goff);
+  const int4 z = make_int4(0, 0, 0, 0);
+  for (int p = 0; p < d.world; p++)
+    for (size_t j = (size_t)blockIdx.x * kThreads + threadIdx.x; j < per; j += stride) ptx::st_na_v4(gz + (size_t)p * per + j, z);
+  // vectors beyond per*world are read by nobody
+  for (size_t j = per * d.world + (size_t)blockIdx.x * kThreads + threadIdx.x; j < nvec; j += stride) ptx::st_na_v4(gz + j, z);
+}
+
+// SGD: one batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch
 // reductions / peer loads, fp32 master + momentum) are issued before any dependent math so that
 // U*(1 + 2*E/4) requests per thread are in flight: the kernel is latency*bandwidth bound
 // (NVLink round trip ~3 us, HBM), not ALU bound.
@@ -439,12 +487,8 @@ __device__ __forceinline__ void fused_sgd_batch(const CollDev& d, size_t goff, s
   float4 pm[U][Q], bm[U][Q];
   float gp2p[(MODE == 2) ? U : 1][8];
 #pragma unroll
-  for (int u = 0; u < U; u++) {
-    const size_t vo = (start + i + u * stride) * 16;
-    if constexpr (MODE == 1) gv[u] = mc_ld_reduce<DT, BNET_SUM>(d.mc + goff + vo);
-    else if constexpr (MODE == 2) p2p_reduce<DT, BNET_SUM>(d, goff + vo, d.rank, gp2p[u]);
-    else gv[u] = ptx::ld_na_v4(reinterpret_cast<const int4*>(d.heap[0] + goff + vo));
-  }
+  for (int u = 0; u < U; u++)
+    fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
 #pragma unroll
   for (int u = 0; u < U; u++) {
     const float4* mp = reinterpret_cast<const float4*>(master + (i + u * stride) * E);
@@ -459,12 +503,7 @@ __device__ __forceinline__ void fused_sgd_batch(const CollDev& d, size_t goff, s
   for (int u = 0; u < U; u++) {
     const size_t vo = (start + i + u * stride) * 16;
     float g[8], p[8], b[8];
-    if constexpr (MODE == 2) {
-#pragma unroll
-      for (int k = 0; k < E; k++) g[k] = gp2p[u][k];
-    } else {
-      unpack<DT>(gv[u], g);
-    }
+    fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
 #pragma unroll
     for (int q = 0; q < Q; q++) {
       p[4 * q] = pm[u][q].x; p[4 * q + 1] = pm[u][q].y; p[4 * q + 2] = pm[u][q].z; p[4 * q + 3] = pm[u][q].w;
@@ -483,18 +522,7 @@ __device__ __forceinline__ void fused_sgd_batch(const CollDev& d, size_t goff, s
       ptx::st_na_f4(mp + q, make_float4(p[4 * q], p[4 * q + 1], p[4 * q + 2], p[4 * q + 3]));
       ptx::st_na_f4(bp + q, make_float4(b[4 * q], b[4 * q + 1], b[4 * q + 2], b[4 * q + 3]));
     }
-    const int4 out = pack<DT>(p);
-    if constexpr (MODE == 1) {
-      ptx::multimem_st_v4(d.mc + poff + vo, out);          // new parameters land on every rank
-    } else if constexpr (MODE == 2) {
-      for (int j = 0; j < d.world; j++) {
-        int pr = d.rank + j;
-        if (pr >= d.world) pr -= d.world;
-        ptx::st_na_v4(reinterpret_cast<int4*>(d.heap[pr] + poff + vo), out);
-      }
-    } else {
-      ptx::st_na_v4(reinterpret_cast<int4*>(d.heap[0] + poff + vo), out);
-    }
+    fused_param_store<MODE>(d, poff + vo, pack<DT>(p));
   }
 }
 
@@ -522,18 +550,64 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_fused_sgd_kernel(CollDev d, 
   for (; i < per; i += stride)
     fused_sgd_batch<DT, MODE, 1>(d, goff, poff, start, i, stride, lr, mu, wd, gscale, master, mom);
   if constexpr (MODE != 0) rank_barrier(d, chan);
-  if (zero_grads) {
-    // Reset our gradients for the next backward.  The barrier above only pairs CTA b with CTA b of the peers (CTAs
-    // of a grid start staggered when the kernel runs under backward on the side stream), so CTA b may only zero
-    // what CTA b of some rank has READ: shard p, vectors p*per + i for exactly the i this CTA walks above.  Zeroing
-    // with a flat index would hand vectors of shard p >= 1 to a different CTA than the one rank p reads them with.
-    int4* gz = reinterpret_cast<int4*>(d.heap[d.rank] + goff);
-    const int4 z = make_int4(0, 0, 0, 0);
-    for (int p = 0; p < d.world; p++)
-      for (size_t j = (size_t)blockIdx.x * kThreads + threadIdx.x; j < per; j += stride) ptx::st_na_v4(gz + (size_t)p * per + j, z);
-    // vectors beyond per*world are read by nobody
-    for (size_t j = per * d.world + (size_t)blockIdx.x * kThreads + threadIdx.x; j < nvec; j += stride) ptx::st_na_v4(gz + j, z);
+  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
+}
+
+// AdamW: one 16-byte gradient vector per thread per iteration, its load (in-switch reduction / peer loads) issued
+// together with the 3*E fp32 state loads before any dependent math.  SGD's two vectors per iteration would hold
+// 2*(3*E + 4) live values for bf16: ptxas spills that at the 64-register cap of two 512-thread CTAs per SM.  One
+// vector fits without spilling and still keeps 1024 threads * (16 + 12*E) bytes of loads in flight per SM.
+template <int DT, int MODE>
+__device__ __forceinline__ void fused_adamw_vec(const CollDev& d, size_t goff, size_t poff, size_t start, size_t i,
+                                                const optim::AdamWCoef& c, float* __restrict__ master,
+                                                float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq) {
+  constexpr int E = VecTraits<DT>::kElems;
+  constexpr int Q = E / 4;
+  int4 gv;
+  float gp2p[8];
+  fused_grad_issue<DT, MODE>(d, goff + (start + i) * 16, gv, gp2p);
+  const size_t e0 = i * E;
+  float4 pm[Q], am[Q], vm[Q];
+#pragma unroll
+  for (int q = 0; q < Q; q++) {
+    pm[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(master + e0) + q);
+    am[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(exp_avg + e0) + q);
+    vm[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(exp_avg_sq + e0) + q);
   }
+  float g[8], p[8], m[8], v[8];
+  fused_grad_get<DT, MODE>(gv, gp2p, g);
+#pragma unroll
+  for (int q = 0; q < Q; q++) {
+    p[4 * q] = pm[q].x; p[4 * q + 1] = pm[q].y; p[4 * q + 2] = pm[q].z; p[4 * q + 3] = pm[q].w;
+    m[4 * q] = am[q].x; m[4 * q + 1] = am[q].y; m[4 * q + 2] = am[q].z; m[4 * q + 3] = am[q].w;
+    v[4 * q] = vm[q].x; v[4 * q + 1] = vm[q].y; v[4 * q + 2] = vm[q].z; v[4 * q + 3] = vm[q].w;
+  }
+#pragma unroll
+  for (int k = 0; k < E; k++) optim::adamw_update(g[k], p[k], m[k], v[k], c);
+#pragma unroll
+  for (int q = 0; q < Q; q++) {
+    ptx::st_na_f4(reinterpret_cast<float4*>(master + e0) + q, make_float4(p[4 * q], p[4 * q + 1], p[4 * q + 2], p[4 * q + 3]));
+    ptx::st_na_f4(reinterpret_cast<float4*>(exp_avg + e0) + q, make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]));
+    ptx::st_na_f4(reinterpret_cast<float4*>(exp_avg_sq + e0) + q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+  }
+  fused_param_store<MODE>(d, poff + (start + i) * 16, pack<DT>(p));
+}
+
+// Same structure as bnet_fused_sgd_kernel; hp: the 8-float block of optim_body.cuh, always read from device memory.
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_fused_adamw_kernel(CollDev d, size_t goff, size_t poff, size_t nvec,
+                                                                   const float* __restrict__ hp, float* __restrict__ master,
+                                                                   float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+                                                                   int zero_grads, int chan) {
+  const optim::AdamWCoef c = optim::adamw_coef(hp);
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  const size_t per = nvec / d.world;
+  const size_t start = (size_t)d.rank * per;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < per; i += stride)
+    fused_adamw_vec<DT, MODE>(d, goff, poff, start, i, c, master, exp_avg, exp_avg_sq);
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
 }
 
 // ------------------------------------------------------------------ multi-tensor pack + cast (K5)
@@ -1080,22 +1154,53 @@ BNET_API int bnet_fused_allreduce_sgd_hp(BnetColl* c, size_t grad_off, size_t pa
                                   nblocks, stream, hp_dev);
 }
 
+// Input checks shared by the fused optimizer entry points (`what` names the optimizer in the message).
+static int fused_check(BnetColl* c, const char* what, size_t grad_off, size_t param_off, size_t count, int dtype, int channel) {
+  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
+  if (dtype != BNET_F32 && dtype != BNET_BF16) return fail("fused %s supports f32 and bf16", what);
+  size_t bytes = count * elsize(dtype);
+  if (bytes % (16 * (size_t)c->world) || grad_off % 16 || param_off % 16) return fail("fused %s needs 16-byte aligned offsets and bytes%%(16*world)==0", what);
+  if (grad_off + bytes > c->alloc_bytes - kPadBytes || param_off + bytes > c->alloc_bytes - kPadBytes) return fail("fused %s range outside the heap", what);
+  return 0;
+}
+
 static int fused_allreduce_sgd_impl(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, float lr,
                                     float momentum, float weight_decay, float grad_scale, float* master, float* mom_buf,
                                     int zero_grads, int channel, int nblocks, void* stream, const float* hp) {
-  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
-  if (dtype != BNET_F32 && dtype != BNET_BF16) return fail("fused SGD supports f32 and bf16");
-  size_t bytes = count * elsize(dtype);
-  if (bytes % (16 * (size_t)c->world) || grad_off % 16 || param_off % 16) return fail("fused SGD needs 16-byte aligned offsets and bytes%%(16*world)==0");
-  if (grad_off + bytes > c->alloc_bytes - kPadBytes || param_off + bytes > c->alloc_bytes - kPadBytes) return fail("fused SGD range outside the heap");
+  if (fused_check(c, "SGD", grad_off, param_off, count, dtype, channel) < 0) return -1;
   if (((uintptr_t)master | (uintptr_t)mom_buf) & 15) return fail("optimizer state must be 16-byte aligned");
   refresh_devp(c);
-  size_t nvec = bytes / 16;
+  size_t nvec = count * elsize(dtype) / 16;
   int nb = pick_blocks(c, nvec / c->world, nblocks, prefer_nvls(c) && env_int("FUSED_NVLS", 1) ? BLK_FUSED_NVLS : BLK_P2P);
   cudaStream_t st = (cudaStream_t)stream;
   size_t goff = kPadBytes + grad_off, poff = kPadBytes + param_off;
   if (dtype == BNET_F32) return run_fused<BNET_F32>(c, goff, poff, nvec, lr, momentum, weight_decay, grad_scale, master, mom_buf, zero_grads, channel, nb, st, hp);
   return run_fused<BNET_BF16>(c, goff, poff, nvec, lr, momentum, weight_decay, grad_scale, master, mom_buf, zero_grads, channel, nb, st, hp);
+}
+
+template <int DT>
+static int run_fused_adamw(BnetColl* c, size_t goff, size_t poff, size_t nvec, const float* hp, float* master, float* m1,
+                           float* m2, int zero, int chan, int nb, cudaStream_t st) {
+  if (c->world == 1)
+    return launch(bnet_fused_adamw_kernel<DT, 0>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
+  if (prefer_nvls(c) && env_int("FUSED_NVLS", 1))
+    return launch(bnet_fused_adamw_kernel<DT, 1>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
+  return launch(bnet_fused_adamw_kernel<DT, 2>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
+}
+
+BNET_API int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype,
+                                        const float* hp_dev, float* master, float* exp_avg, float* exp_avg_sq, int zero_grads,
+                                        int channel, int nblocks, void* stream) {
+  if (fused_check(c, "AdamW", grad_off, param_off, count, dtype, channel) < 0) return -1;
+  if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (((uintptr_t)master | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) return fail("optimizer state must be 16-byte aligned");
+  refresh_devp(c);
+  size_t nvec = count * elsize(dtype) / 16;
+  int nb = pick_blocks(c, nvec / c->world, nblocks, prefer_nvls(c) && env_int("FUSED_NVLS", 1) ? BLK_FUSED_NVLS : BLK_P2P);
+  cudaStream_t st = (cudaStream_t)stream;
+  size_t goff = kPadBytes + grad_off, poff = kPadBytes + param_off;
+  if (dtype == BNET_F32) return run_fused_adamw<BNET_F32>(c, goff, poff, nvec, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel, nb, st);
+  return run_fused_adamw<BNET_BF16>(c, goff, poff, nvec, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel, nb, st);
 }
 
 BNET_API int bnet_pack_cast(const BnetPackItem* items_dev, int n, void* dst, int src_dtype, int dst_dtype, float scale,

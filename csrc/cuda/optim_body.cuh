@@ -1,0 +1,67 @@
+// Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu).
+//
+// The update is written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into
+// bnet_fused_adamw_kernel by nvcc and (b) compiled by g++ and checked against a long-double AdamW by
+// csrc/tests/optim_emu_test.cc, without a GPU.  Every product that feeds a sum is an explicit fmaf, so nvcc's
+// contraction and g++'s lack of it cannot make the two builds round differently.
+#pragma once
+#include <math.h>
+
+#if defined(__CUDACC__)
+#define BNET_OPT_HD __host__ __device__ __forceinline__
+#else
+#define BNET_OPT_HD inline
+#endif
+
+namespace bnet {
+namespace optim {
+
+// Hyper-parameter block of the fused AdamW kernel: 8 floats of device memory, 16-byte aligned, read when the kernel
+// runs, so a captured CUDA graph follows a learning-rate schedule and the bias correction without being re-captured.
+// `step` counts the steps already taken (the kernel uses t = step + 1).  A float counts exactly up to 2^24 steps.
+enum { kHpLr = 0, kHpBeta1, kHpBeta2, kHpEps, kHpWeightDecay, kHpGradScale, kHpStep, kHpReserved, kHpWords };
+
+struct AdamWCoef {
+  float decay;       // 1 - lr * weight_decay
+  float beta1, omb1; // beta1, 1 - beta1
+  float beta2, omb2; // beta2, 1 - beta2
+  float step_size;   // lr / (1 - beta1^t)
+  float bc2_sqrt;    // sqrt(1 - beta2^t)
+  float eps, gscale;
+};
+
+// The bias corrections are taken in double: 1 - beta2^t at t = 1 is a difference of nearly equal numbers, and
+// fp32 powf would cost it up to ~1e-4 of relative accuracy.  This runs once per thread, not per element.
+BNET_OPT_HD AdamWCoef adamw_coef(const float* hp) {
+  AdamWCoef c;
+  const double lr = hp[kHpLr], b1 = hp[kHpBeta1], b2 = hp[kHpBeta2];
+  const double t = (double)hp[kHpStep] + 1.0;
+  c.decay = (float)(1.0 - lr * (double)hp[kHpWeightDecay]);
+  c.beta1 = hp[kHpBeta1];
+  c.omb1 = (float)(1.0 - b1);
+  c.beta2 = hp[kHpBeta2];
+  c.omb2 = (float)(1.0 - b2);
+  c.step_size = (float)(lr / (1.0 - pow(b1, t)));
+  c.bc2_sqrt = (float)sqrt(1.0 - pow(b2, t));
+  c.eps = hp[kHpEps];
+  c.gscale = hp[kHpGradScale];
+  return c;
+}
+
+// One element of torch.optim.AdamW (amsgrad=False, maximize=False), in the order of torch's fused CUDA kernel:
+//   g = grad * gscale;  p *= 1 - lr*wd;  m = b1*m + (1-b1)*g;  v = b2*v + (1-b2)*g*g;
+//   p -= step_size * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
+// IEEE arithmetic carries NaN and Inf where torch's does: a NaN gradient makes this element's p, m and v NaN; an
+// infinite one makes m and v infinite and p NaN (inf / inf).  |g| beyond ~1.8e19 overflows g*g in fp32, as it does
+// in torch's fp32 state.
+BNET_OPT_HD void adamw_update(float grad, float& p, float& m, float& v, const AdamWCoef& c) {
+  const float g = grad * c.gscale;
+  p = p * c.decay;
+  m = fmaf(c.beta1, m, c.omb1 * g);
+  v = fmaf(c.beta2, v, (c.omb2 * g) * g);
+  const float denom = sqrtf(v) / c.bc2_sqrt + c.eps;
+  p = fmaf(-c.step_size, m / denom, p);
+}
+
+}  // namespace optim
+}  // namespace bnet

@@ -84,6 +84,18 @@ int bnet_fused_allreduce_sgd(BnetColl* c, size_t grad_off, size_t param_off, siz
  * kernel runs: a captured CUDA graph follows a learning-rate schedule without being re-captured. */
 int bnet_fused_allreduce_sgd_hp(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, const float* hp_dev,
                                 float* master, float* mom_buf, int zero_grads, int channel, int nblocks, void* stream);
+/* Fused gradient all-reduce + AdamW (decoupled weight decay, torch.optim.AdamW semantics without amsgrad / maximize) +
+ * parameter broadcast, one kernel, laid out like bnet_fused_allreduce_sgd.  Per element of the owner's shard, with
+ * g = sum over ranks of grad * grad_scale and t = step + 1:
+ *   p = p*(1 - lr*wd);  m = b1*m + (1-b1)*g;  v = b2*v + (1-b2)*g*g;  p -= lr/(1-b1^t) * m / (sqrt(v)/sqrt(1-b2^t) + eps)
+ * hp_dev: 8 floats of device memory, 16-byte aligned, read when the kernel runs:
+ *   {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved}
+ * `step` is the number of steps already taken; the caller advances it once per training step (not per bucket), so a
+ * captured CUDA graph follows the schedule and the bias correction.  A float counts steps exactly up to 2^24.
+ * master/exp_avg/exp_avg_sq: local fp32 arrays of count/world elements (this rank's shard), 16-byte aligned. */
+int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, const float* hp_dev,
+                               float* master, float* exp_avg, float* exp_avg_sq, int zero_grads, int channel, int nblocks,
+                               void* stream);
 
 /* Multi-tensor pack+cast into the heap (K5): n tensors described on the device. */
 typedef struct {
