@@ -241,23 +241,9 @@ class SymmComm:
         (``master``/``mom``: numel/world each) and write the new ``param`` on every rank.
         ``hp``: optional 4-element fp32 CUDA tensor {lr, momentum, weight_decay, grad_scale} that the kernel reads when
         it runs (overrides the scalar arguments) — lets a captured CUDA graph follow a learning-rate schedule."""
-        assert grad.numel() == param.numel() and grad.dtype == param.dtype
-        assert master.dtype == torch.float32 and mom.dtype == torch.float32
-        assert master.numel() * self.world == grad.numel() == mom.numel() * self.world
-        if hp is not None:
-            assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= 4 and hp.is_contiguous()
-            n = self._chk(self.lib.bnet_fused_allreduce_sgd_hp(
-                self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], C.c_void_p(hp.data_ptr()),
-                C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), 1 if zero_grads else 0, channel, nblocks,
-                self._stream(stream)), "fused_allreduce_sgd_hp")
-            self.launches += n
-            return
         gs = (1.0 / self.world) if grad_scale is None else grad_scale
-        n = self._chk(self.lib.bnet_fused_allreduce_sgd(
-            self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], lr, momentum,
-            weight_decay, gs, C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), 1 if zero_grads else 0,
-            channel, nblocks, self._stream(stream)), "fused_allreduce_sgd")
-        self.launches += n
+        self._fused_step("fused_allreduce_sgd" if hp is None else "fused_allreduce_sgd_hp", grad, param, (master, mom),
+                         (lr, momentum, weight_decay, gs), hp, 4, zero_grads, channel, nblocks, stream)
 
     def fused_allreduce_adamw(self, grad: torch.Tensor, param: torch.Tensor, master: torch.Tensor, exp_avg: torch.Tensor,
                               exp_avg_sq: torch.Tensor, hp: torch.Tensor, zero_grads: bool = True, channel: int = 0,
@@ -266,16 +252,22 @@ class SymmComm:
         ``exp_avg_sq``: numel/world each) and write the new ``param`` on every rank.  ``hp``: fp32 CUDA tensor of 8
         elements {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved} that the kernel reads when it runs;
         ``step`` counts the steps already taken and is not advanced here (the caller does that once per step)."""
-        assert grad.numel() == param.numel() and grad.dtype == param.dtype
-        assert master.dtype == exp_avg.dtype == exp_avg_sq.dtype == torch.float32
-        assert master.numel() * self.world == grad.numel() == exp_avg.numel() * self.world == exp_avg_sq.numel() * self.world
-        assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= 8 and hp.is_contiguous()
-        n = self._chk(self.lib.bnet_fused_allreduce_adamw(
-            self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], C.c_void_p(hp.data_ptr()),
-            C.c_void_p(master.data_ptr()), C.c_void_p(exp_avg.data_ptr()), C.c_void_p(exp_avg_sq.data_ptr()),
-            1 if zero_grads else 0, channel, nblocks, self._stream(stream)), "fused_allreduce_adamw")
-        self.launches += n
+        assert hp is not None
+        self._fused_step("fused_allreduce_adamw", grad, param, (master, exp_avg, exp_avg_sq), (), hp, 8, zero_grads, channel,
+                         nblocks, stream)
 
+    def _fused_step(self, name, grad, param, state, scalars, hp, hp_words, zero_grads, channel, nblocks, stream):
+        """Calls ``bnet_<name>``: the checks both fused optimizers share.  ``state``: the fp32 shards, master first;
+        ``hp``: the device hyper-parameter block of at least ``hp_words`` floats, passed instead of ``scalars``."""
+        assert grad.numel() == param.numel() and grad.dtype == param.dtype
+        assert all(s.dtype == torch.float32 and s.numel() * self.world == grad.numel() for s in state)
+        if hp is not None:
+            assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= hp_words and hp.is_contiguous()
+            scalars = (C.c_void_p(hp.data_ptr()),)
+        n = self._chk(getattr(self.lib, "bnet_" + name)(
+            self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], *scalars,
+            *(C.c_void_p(s.data_ptr()) for s in state), 1 if zero_grads else 0, channel, nblocks, self._stream(stream)), name)
+        self.launches += n
 
     # ------------------------------------------------------------------ collectives on ordinary tensors
     # The kernels above work on heap tensors in place.  These wrappers accept any CUDA tensor: they stage it

@@ -132,14 +132,22 @@ def direct_grads_self_check(device=None, group=None, steps: int = 3, make_model=
     return ok, detail
 
 
+# The fp32 tensors the fused kernel updates in every bucket's shard, master weights first; also their state-dict keys.
+_STATE_NAMES = {"sgd": ("master", "momentum"), "adamw": ("master", "exp_avg", "exp_avg_sq")}
+
+
 class _Bucket:
-    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "master", "mom", "exp_avg", "exp_avg_sq")
+    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state")
 
     def __init__(self):
         self.params = []
         self.start = 0
         self.numel = 0
         self.ready = 0
+
+    @property
+    def master(self) -> torch.Tensor:
+        return self.state[0]
 
 
 class BnetDDP(torch.nn.Module):
@@ -259,15 +267,11 @@ class BnetDDP(torch.nn.Module):
             b.grad = self.flat_grad[b.start:b.start + b.numel]
             b.param = self.flat_param[b.start:b.start + b.numel]
             shard = b.numel // comm.world
-            b.master = b.param[comm.rank * shard:(comm.rank + 1) * shard].float().contiguous()
-            if optimizer == "adamw":
-                b.exp_avg = torch.zeros_like(b.master)
-                b.exp_avg_sq = torch.zeros_like(b.master)
-            else:
-                b.mom = torch.zeros_like(b.master)
-        if optimizer == "adamw":
-            # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh)
-            self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev)
+            master = b.param[comm.rank * shard:(comm.rank + 1) * shard].float().contiguous()
+            b.state = (master,) + tuple(torch.zeros_like(master) for _ in _STATE_NAMES[optimizer][1:])
+        # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh); SGD
+        # passes them as launch arguments until the first set_lr
+        self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev) if optimizer == "adamw" else None
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad) for p in params]
@@ -297,12 +301,12 @@ class BnetDDP(torch.nn.Module):
         ev.record(cur)
         self.comm_stream.wait_event(ev)          # the bucket's gradients are complete on the compute stream
         if self.optimizer == "adamw":
-            self.comm.fused_allreduce_adamw(b.grad, b.param, b.master, b.exp_avg, b.exp_avg_sq, self._hp, zero_grads=True,
-                                            channel=0, nblocks=self.nblocks, stream=self.comm_stream)
+            self.comm.fused_allreduce_adamw(b.grad, b.param, *b.state, self._hp, zero_grads=True, channel=0,
+                                            nblocks=self.nblocks, stream=self.comm_stream)
         else:
-            self.comm.fused_allreduce_sgd(b.grad, b.param, b.master, b.mom, self.lr, self.momentum, self.weight_decay,
+            self.comm.fused_allreduce_sgd(b.grad, b.param, *b.state, self.lr, self.momentum, self.weight_decay,
                                           zero_grads=True, channel=0, nblocks=self.nblocks, stream=self.comm_stream,
-                                          hp=getattr(self, "_hp", None))
+                                          hp=self._hp)
         b.ready = 0
         self._inflight = True
 
@@ -350,29 +354,22 @@ class BnetDDP(torch.nn.Module):
         with torch.cuda.stream(side):               # warm-up on a side stream (cuDNN autotune, allocator)
             # The warm-up runs REAL steps (the fused optimizer included: every rank has to take part in its
             # barriers), so everything a step mutates is saved first and put back afterwards — parameters, fp32
-            # master weights, momentum, module buffers (BatchNorm running statistics).  A (re)capture therefore
-            # leaves the training trajectory exactly where eager mode would have it; checkpoint/resume stays
-            # step-exact.
-            saved = [self.flat_param.clone()] + [t.clone() for b in self.buckets for t in self._state(b)]
-            if self.optimizer == "adamw":
-                saved.append(self._hp.clone())      # (the step count)
-            bufs = [t for t in self.module.buffers() if t.is_cuda and t.numel()]
-            saved_bufs = [t.clone() for t in bufs]
+            # optimizer state, the hyper-parameter block (AdamW's step count), module buffers (BatchNorm running
+            # statistics).  A (re)capture therefore leaves the training trajectory exactly where eager mode would
+            # have it; checkpoint/resume stays step-exact.
+            live = [self.flat_param] + [t for b in self.buckets for t in b.state]
+            live += [t for t in self.module.buffers() if t.is_cuda and t.numel()]
+            if self._hp is not None:
+                live.append(self._hp)
+            saved = [t.clone() for t in live]
             for _ in range(2):
                 self._eager_step(self._gx, self._gy, loss_fn)
             torch.cuda.current_stream().synchronize()
             if self.comm.world > 1:
                 dist.barrier()                      # nobody restores while a peer's kernel still writes parameters
-            it = iter(saved)
-            self.flat_param.copy_(next(it))
-            for b in self.buckets:
-                for t in self._state(b):
-                    t.copy_(next(it))
-            if self.optimizer == "adamw":
-                self._hp.copy_(next(it))
-            for t, s in zip(bufs, saved_bufs):
+            for t, s in zip(live, saved):
                 t.copy_(s)
-            del saved, saved_bufs
+            del live, saved
         cur.wait_stream(side)
         torch.cuda.synchronize()
         if self.comm.world > 1:
@@ -397,7 +394,7 @@ class BnetDDP(torch.nn.Module):
         from ..ops import fused_nn
 
         # with the hyper-parameters in device memory (after the first set_lr) the captured step does not depend on them
-        hpkey = "device" if getattr(self, "_hp", None) is not None else (self.lr, self.momentum, self.weight_decay)
+        hpkey = "device" if self._hp is not None else (self.lr, self.momentum, self.weight_decay)
         # (a lambda written inline is a new function object every call, but always the same code object)
         fn_key = (getattr(loss_fn, "__code__", loss_fn), getattr(loss_fn, "__closure__", None) is None or id(loss_fn))
         key = (tuple(inputs.shape), inputs.dtype, tuple(targets.shape), targets.dtype, fn_key, hpkey)
@@ -492,14 +489,13 @@ class BnetDDP(torch.nn.Module):
     # weights and momentum (SGD) or exp_avg / exp_avg_sq (AdamW, which also saves its step count) of every bucket.
     def optimizer_state_dict(self) -> dict:
         if self.optimizer == "adamw":
-            return {"optimizer": "adamw", "lr": self.lr, "betas": self.betas, "eps": self.eps,
-                    "weight_decay": self.weight_decay, "step": int(self._hp[self._HP_STEP].item()),
-                    "world": self.comm.world, "rank": self.comm.rank,
-                    "buckets": [{"master": b.master.detach().cpu(), "exp_avg": b.exp_avg.detach().cpu(),
-                                 "exp_avg_sq": b.exp_avg_sq.detach().cpu()} for b in self.buckets]}
-        return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay,
-                "world": self.comm.world, "rank": self.comm.rank,
-                "buckets": [{"master": b.master.detach().cpu(), "momentum": b.mom.detach().cpu()} for b in self.buckets]}
+            head = {"optimizer": "adamw", "lr": self.lr, "betas": self.betas, "eps": self.eps,
+                    "weight_decay": self.weight_decay, "step": int(self._hp[self._HP_STEP].item())}
+        else:
+            head = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
+        names = _STATE_NAMES[self.optimizer]
+        return {**head, "world": self.comm.world, "rank": self.comm.rank,
+                "buckets": [{k: t.detach().cpu() for k, t in zip(names, b.state)} for b in self.buckets]}
 
     def load_optimizer_state_dict(self, state: dict) -> None:
         kind = state.get("optimizer", "sgd")
@@ -510,19 +506,15 @@ class BnetDDP(torch.nn.Module):
         for b, s in zip(self.buckets, state["buckets"]):
             if s["master"].shape != b.master.shape:
                 raise ValueError("optimizer state shard does not match this bucket")
-            b.master.copy_(s["master"])
-            if self.optimizer == "adamw":
-                b.exp_avg.copy_(s["exp_avg"])
-                b.exp_avg_sq.copy_(s["exp_avg_sq"])
-            else:
-                b.mom.copy_(s["momentum"])
+            for k, t in zip(_STATE_NAMES[self.optimizer], b.state):
+                t.copy_(s[k])
         if self.optimizer == "adamw":
             self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
             self.betas = tuple(state["betas"])
             self._hp.copy_(torch.tensor(self._adamw_hp(state["step"]), dtype=torch.float32))
             return
         self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
-        if getattr(self, "_hp", None) is not None:
+        if self._hp is not None:
             self.set_lr(self.lr)              # hyper-parameters live in device memory: refresh them
         else:
             self._graph = None                # hyper-parameters are baked into a captured step
@@ -563,7 +555,7 @@ class BnetDDP(torch.nn.Module):
         if weight_decay is not None:
             self.weight_decay = float(weight_decay)
         vals = [self.lr, self.momentum, self.weight_decay, 1.0 / self.comm.world]
-        if getattr(self, "_hp", None) is None:
+        if self._hp is None:
             self._hp = torch.tensor(vals, dtype=torch.float32, device=self.flat_param.device)
             self._graph = None
         else:
@@ -576,8 +568,8 @@ class BnetDDP(torch.nn.Module):
         return [self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, 1.0 / self.comm.world, float(step), 0.0]
 
     def _state(self, b: _Bucket) -> tuple:
-        """The fp32 tensors the fused kernel updates for bucket `b`."""
-        return (b.master, b.exp_avg, b.exp_avg_sq) if self.optimizer == "adamw" else (b.master, b.mom)
+        """The fp32 tensors the fused kernel updates for bucket `b`, master first."""
+        return b.state
 
     @property
     def kernel_launches(self) -> int:

@@ -426,8 +426,8 @@ __global__ void __launch_bounds__(256) bnet_allreduce_ll_kernel(CollDev d, size_
 // ------------------------------------------------------------------ fused all-reduce + optimizer + broadcast
 // MODE 0: single GPU, 1: NVLS multicast, 2: peer loads/stores
 //
-// Shared by the SGD and AdamW kernels: the summed gradient vector at heap byte offset `go` (MODE 1: in-switch
-// reduction, raw vector in gv; MODE 2: peer loads summed in fp32 into gf; MODE 0: the local vector in gv) ...
+// The summed gradient vector at heap byte offset `go` (MODE 1: in-switch reduction, raw vector in gv; MODE 2: peer
+// loads summed in fp32 into gf; MODE 0: the local vector in gv) ...
 template <int DT, int MODE>
 __device__ __forceinline__ void fused_grad_issue(const CollDev& d, size_t go, int4& gv, float* gf) {
   if constexpr (MODE == 1) gv = mc_ld_reduce<DT, BNET_SUM>(d.mc + go);
@@ -473,57 +473,86 @@ __device__ __forceinline__ void fused_zero_grads(const CollDev& d, size_t goff, 
   for (size_t j = per * d.world + (size_t)blockIdx.x * kThreads + threadIdx.x; j < nvec; j += stride) ptx::st_na_v4(gz + j, z);
 }
 
-// SGD: one batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch
-// reductions / peer loads, fp32 master + momentum) are issued before any dependent math so that
-// U*(1 + 2*E/4) requests per thread are in flight: the kernel is latency*bandwidth bound
-// (NVLink round trip ~3 us, HBM), not ALU bound.
-template <int DT, int MODE, int U>
-__device__ __forceinline__ void fused_sgd_batch(const CollDev& d, size_t goff, size_t poff, size_t start, size_t i,
-                                                size_t stride, float lr, float mu, float wd, float gscale,
-                                                float* __restrict__ master, float* __restrict__ mom) {
+// Optimizer policies of the fused step: kStates fp32 arrays per element (master weights first), kU gradient vectors
+// per thread per batch, and the per-element update of optim_body.cuh.
+struct SgdOpt {
+  static constexpr int kStates = 2;   // master, momentum
+  static constexpr int kU = 2;        // (register budget: 2 CTAs/SM)
+  float lr, mu, wd, gscale;
+  __device__ __forceinline__ void update(float g, float (&s)[kStates][8], int k) const {
+    optim::sgd_update(g, s[0][k], s[1][k], lr, mu, wd, gscale);
+  }
+};
+// AdamW takes one vector per batch: two would hold 2*(3*E + 4) live values for bf16, and ptxas spills that at the
+// 64-register cap of two 512-thread CTAs per SM.  One vector fits without spilling and still keeps
+// 1024 threads * (16 + 12*E) bytes of loads in flight per SM.
+struct AdamWOpt {
+  static constexpr int kStates = 3;   // master, exp_avg, exp_avg_sq
+  static constexpr int kU = 1;
+  optim::AdamWCoef c;
+  __device__ __forceinline__ void update(float g, float (&s)[kStates][8], int k) const {
+    optim::adamw_update(g, s[0][k], s[1][k], s[2][k], c);
+  }
+};
+
+// One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch reductions / peer loads, the
+// fp32 state) are issued before any dependent math so that U*(1 + S*E/4) requests per thread are in flight: the
+// kernel is latency*bandwidth bound (NVLink round trip ~3 us, HBM), not ALU bound.
+template <int DT, int MODE, int U, class Opt>
+__device__ __forceinline__ void fused_batch(const CollDev& d, size_t goff, size_t poff, size_t start, size_t i, size_t stride,
+                                            const Opt& opt, float* const (&state)[Opt::kStates]) {
   constexpr int E = VecTraits<DT>::kElems;
   constexpr int Q = E / 4;
+  constexpr int S = Opt::kStates;
   int4 gv[U];
-  float4 pm[U][Q], bm[U][Q];
+  float4 sm[U][S][Q];
   float gp2p[(MODE == 2) ? U : 1][8];
 #pragma unroll
   for (int u = 0; u < U; u++)
     fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
 #pragma unroll
-  for (int u = 0; u < U; u++) {
-    const float4* mp = reinterpret_cast<const float4*>(master + (i + u * stride) * E);
-    const float4* bp = reinterpret_cast<const float4*>(mom + (i + u * stride) * E);
+  for (int u = 0; u < U; u++)
 #pragma unroll
-    for (int q = 0; q < Q; q++) {
-      pm[u][q] = ptx::ld_na_f4(mp + q);
-      bm[u][q] = ptx::ld_na_f4(bp + q);
-    }
-  }
+    for (int q = 0; q < Q; q++)
+#pragma unroll
+      for (int s = 0; s < S; s++) sm[u][s][q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(state[s] + (i + u * stride) * E) + q);
 #pragma unroll
   for (int u = 0; u < U; u++) {
-    const size_t vo = (start + i + u * stride) * 16;
-    float g[8], p[8], b[8];
+    float g[8], st[S][8];
     fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
 #pragma unroll
-    for (int q = 0; q < Q; q++) {
-      p[4 * q] = pm[u][q].x; p[4 * q + 1] = pm[u][q].y; p[4 * q + 2] = pm[u][q].z; p[4 * q + 3] = pm[u][q].w;
-      b[4 * q] = bm[u][q].x; b[4 * q + 1] = bm[u][q].y; b[4 * q + 2] = bm[u][q].z; b[4 * q + 3] = bm[u][q].w;
-    }
+    for (int q = 0; q < Q; q++)
 #pragma unroll
-    for (int k = 0; k < E; k++) {
-      float dp = fmaf(wd, p[k], g[k] * gscale);   // d_p = g/world + wd*p
-      b[k] = fmaf(mu, b[k], dp);                  // buf = mu*buf + d_p
-      p[k] = fmaf(-lr, b[k], p[k]);               // p  -= lr*buf
-    }
-    float4* mp = reinterpret_cast<float4*>(master + (i + u * stride) * E);
-    float4* bp = reinterpret_cast<float4*>(mom + (i + u * stride) * E);
+      for (int s = 0; s < S; s++) {
+        st[s][4 * q] = sm[u][s][q].x; st[s][4 * q + 1] = sm[u][s][q].y; st[s][4 * q + 2] = sm[u][s][q].z; st[s][4 * q + 3] = sm[u][s][q].w;
+      }
 #pragma unroll
-    for (int q = 0; q < Q; q++) {
-      ptx::st_na_f4(mp + q, make_float4(p[4 * q], p[4 * q + 1], p[4 * q + 2], p[4 * q + 3]));
-      ptx::st_na_f4(bp + q, make_float4(b[4 * q], b[4 * q + 1], b[4 * q + 2], b[4 * q + 3]));
-    }
-    fused_param_store<MODE>(d, poff + vo, pack<DT>(p));
+    for (int k = 0; k < E; k++) opt.update(g[k], st, k);
+#pragma unroll
+    for (int q = 0; q < Q; q++)
+#pragma unroll
+      for (int s = 0; s < S; s++)
+        ptx::st_na_f4(reinterpret_cast<float4*>(state[s] + (i + u * stride) * E) + q,
+                      make_float4(st[s][4 * q], st[s][4 * q + 1], st[s][4 * q + 2], st[s][4 * q + 3]));
+    fused_param_store<MODE>(d, poff + (start + i + u * stride) * 16, pack<DT>(st[0]));
   }
+}
+
+// barrier, reduce + update + broadcast of this rank's shard, barrier, gradient zeroing
+template <int DT, int MODE, class Opt>
+__device__ __forceinline__ void fused_step(const CollDev& d, size_t goff, size_t poff, size_t nvec, const Opt& opt,
+                                           float* const (&state)[Opt::kStates], int zero_grads, int chan) {
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  const size_t per = nvec / d.world;
+  const size_t start = (size_t)d.rank * per;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  constexpr int U = Opt::kU;
+  size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+  for (; i + (U - 1) * stride < per; i += U * stride) fused_batch<DT, MODE, U>(d, goff, poff, start, i, stride, opt, state);
+  if constexpr (U > 1)
+    for (; i < per; i += stride) fused_batch<DT, MODE, 1>(d, goff, poff, start, i, stride, opt, state);
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
 }
 
 template <int DT, int MODE>
@@ -539,75 +568,18 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_fused_sgd_kernel(CollDev d, 
     wd = hp[2];
     gscale = hp[3];
   }
-  if constexpr (MODE != 0) rank_barrier(d, chan);
-  const size_t per = nvec / d.world;
-  const size_t start = (size_t)d.rank * per;
-  const size_t stride = (size_t)gridDim.x * kThreads;
-  constexpr int U = 2;   // 16-byte gradient vectors per thread per batch (register budget: 2 CTAs/SM)
-  size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  for (; i + (U - 1) * stride < per; i += U * stride)
-    fused_sgd_batch<DT, MODE, U>(d, goff, poff, start, i, stride, lr, mu, wd, gscale, master, mom);
-  for (; i < per; i += stride)
-    fused_sgd_batch<DT, MODE, 1>(d, goff, poff, start, i, stride, lr, mu, wd, gscale, master, mom);
-  if constexpr (MODE != 0) rank_barrier(d, chan);
-  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
+  float* const state[2] = {master, mom};
+  fused_step<DT, MODE>(d, goff, poff, nvec, SgdOpt{lr, mu, wd, gscale}, state, zero_grads, chan);
 }
 
-// AdamW: one 16-byte gradient vector per thread per iteration, its load (in-switch reduction / peer loads) issued
-// together with the 3*E fp32 state loads before any dependent math.  SGD's two vectors per iteration would hold
-// 2*(3*E + 4) live values for bf16: ptxas spills that at the 64-register cap of two 512-thread CTAs per SM.  One
-// vector fits without spilling and still keeps 1024 threads * (16 + 12*E) bytes of loads in flight per SM.
-template <int DT, int MODE>
-__device__ __forceinline__ void fused_adamw_vec(const CollDev& d, size_t goff, size_t poff, size_t start, size_t i,
-                                                const optim::AdamWCoef& c, float* __restrict__ master,
-                                                float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq) {
-  constexpr int E = VecTraits<DT>::kElems;
-  constexpr int Q = E / 4;
-  int4 gv;
-  float gp2p[8];
-  fused_grad_issue<DT, MODE>(d, goff + (start + i) * 16, gv, gp2p);
-  const size_t e0 = i * E;
-  float4 pm[Q], am[Q], vm[Q];
-#pragma unroll
-  for (int q = 0; q < Q; q++) {
-    pm[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(master + e0) + q);
-    am[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(exp_avg + e0) + q);
-    vm[q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(exp_avg_sq + e0) + q);
-  }
-  float g[8], p[8], m[8], v[8];
-  fused_grad_get<DT, MODE>(gv, gp2p, g);
-#pragma unroll
-  for (int q = 0; q < Q; q++) {
-    p[4 * q] = pm[q].x; p[4 * q + 1] = pm[q].y; p[4 * q + 2] = pm[q].z; p[4 * q + 3] = pm[q].w;
-    m[4 * q] = am[q].x; m[4 * q + 1] = am[q].y; m[4 * q + 2] = am[q].z; m[4 * q + 3] = am[q].w;
-    v[4 * q] = vm[q].x; v[4 * q + 1] = vm[q].y; v[4 * q + 2] = vm[q].z; v[4 * q + 3] = vm[q].w;
-  }
-#pragma unroll
-  for (int k = 0; k < E; k++) optim::adamw_update(g[k], p[k], m[k], v[k], c);
-#pragma unroll
-  for (int q = 0; q < Q; q++) {
-    ptx::st_na_f4(reinterpret_cast<float4*>(master + e0) + q, make_float4(p[4 * q], p[4 * q + 1], p[4 * q + 2], p[4 * q + 3]));
-    ptx::st_na_f4(reinterpret_cast<float4*>(exp_avg + e0) + q, make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]));
-    ptx::st_na_f4(reinterpret_cast<float4*>(exp_avg_sq + e0) + q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
-  }
-  fused_param_store<MODE>(d, poff + (start + i) * 16, pack<DT>(p));
-}
-
-// Same structure as bnet_fused_sgd_kernel; hp: the 8-float block of optim_body.cuh, always read from device memory.
+// hp: the 8-float block of optim_body.cuh, always read from device memory.
 template <int DT, int MODE>
 __global__ void __launch_bounds__(kThreads, 2) bnet_fused_adamw_kernel(CollDev d, size_t goff, size_t poff, size_t nvec,
                                                                    const float* __restrict__ hp, float* __restrict__ master,
                                                                    float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                                    int zero_grads, int chan) {
-  const optim::AdamWCoef c = optim::adamw_coef(hp);
-  if constexpr (MODE != 0) rank_barrier(d, chan);
-  const size_t per = nvec / d.world;
-  const size_t start = (size_t)d.rank * per;
-  const size_t stride = (size_t)gridDim.x * kThreads;
-  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < per; i += stride)
-    fused_adamw_vec<DT, MODE>(d, goff, poff, start, i, c, master, exp_avg, exp_avg_sq);
-  if constexpr (MODE != 0) rank_barrier(d, chan);
-  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
+  float* const state[3] = {master, exp_avg, exp_avg_sq};
+  fused_step<DT, MODE>(d, goff, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, zero_grads, chan);
 }
 
 // ------------------------------------------------------------------ multi-tensor pack + cast (K5)
@@ -1124,25 +1096,61 @@ BNET_API int bnet_barrier(BnetColl* c, int channel, void* stream) {
   return launch(bnet_barrier_kernel, 1, kThreads, (cudaStream_t)stream, c->devp, channel);
 }
 
-template <int DT>
-static int run_fused(BnetColl* c, size_t goff, size_t poff, size_t nvec, float lr, float mu, float wd, float gs,
-                     float* master, float* mom, int zero, int chan, int nb, cudaStream_t st, const float* hp) {
-  if (c->world == 1)
-    return launch(bnet_fused_sgd_kernel<DT, 0>, nb, kThreads, st, c->devp, goff, poff, nvec, lr, mu, wd, gs, master, mom, zero, chan, hp);
-  if (prefer_nvls(c) && env_int("FUSED_NVLS", 1))
-    return launch(bnet_fused_sgd_kernel<DT, 1>, nb, kThreads, st, c->devp, goff, poff, nvec, lr, mu, wd, gs, master, mom, zero, chan, hp);
-  return launch(bnet_fused_sgd_kernel<DT, 2>, nb, kThreads, st, c->devp, goff, poff, nvec, lr, mu, wd, gs, master, mom, zero, chan, hp);
+// Each optimizer's fused kernel, by dtype and MODE
+struct SgdKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_fused_sgd_kernel<DT, MODE>;
+};
+struct AdamWKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_fused_adamw_kernel<DT, MODE>;
+};
+
+// What a fused optimizer launch needs once its input has been checked
+struct FusedLaunch {
+  size_t goff, poff, nvec;   // heap byte offsets of gradients and parameters, 16-byte vectors in the bucket
+  bool nvls;                 // in-switch reduction (MODE 1) when there is more than one rank
+  int nb;
+  cudaStream_t st;
+};
+
+// Input checks and launch set-up of the fused optimizer entry points: `what` names the optimizer in the messages,
+// `state` lists its fp32 arrays.
+static int fused_prologue(BnetColl* c, const char* what, size_t grad_off, size_t param_off, size_t count, int dtype,
+                          int channel, std::initializer_list<const float*> state, int nblocks, void* stream, FusedLaunch& f) {
+  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
+  if (dtype != BNET_F32 && dtype != BNET_BF16) return fail("fused %s supports f32 and bf16", what);
+  size_t bytes = count * elsize(dtype);
+  if (bytes % (16 * (size_t)c->world) || grad_off % 16 || param_off % 16) return fail("fused %s needs 16-byte aligned offsets and bytes%%(16*world)==0", what);
+  if (grad_off + bytes > c->alloc_bytes - kPadBytes || param_off + bytes > c->alloc_bytes - kPadBytes) return fail("fused %s range outside the heap", what);
+  uintptr_t addr = 0;
+  for (const float* s : state) addr |= (uintptr_t)s;
+  if (addr & 15) return fail("optimizer state must be 16-byte aligned");
+  refresh_devp(c);
+  f.goff = kPadBytes + grad_off;
+  f.poff = kPadBytes + param_off;
+  f.nvec = bytes / 16;
+  f.nvls = prefer_nvls(c) && env_int("FUSED_NVLS", 1);
+  f.nb = pick_blocks(c, f.nvec / c->world, nblocks, f.nvls ? BLK_FUSED_NVLS : BLK_P2P);
+  f.st = (cudaStream_t)stream;
+  return 0;
 }
 
-static int fused_allreduce_sgd_impl(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, float lr,
-                                    float momentum, float weight_decay, float grad_scale, float* master, float* mom_buf,
-                                    int zero_grads, int channel, int nblocks, void* stream, const float* hp);
+// Launches K's kernel for `dtype` in MODE 0 on one GPU, 1 with NVLS, 2 with peer loads and stores.
+template <class K, typename... A>
+static int run_fused(BnetColl* c, int dtype, const FusedLaunch& f, A... args) {
+  const int mode = c->world == 1 ? 0 : f.nvls ? 1 : 2;
+  const std::decay_t<decltype(K::template fn<BNET_F32, 0>)> kern[2][3] = {
+      {K::template fn<BNET_F32, 0>, K::template fn<BNET_F32, 1>, K::template fn<BNET_F32, 2>},
+      {K::template fn<BNET_BF16, 0>, K::template fn<BNET_BF16, 1>, K::template fn<BNET_BF16, 2>}};
+  return launch(kern[dtype == BNET_BF16][mode], f.nb, kThreads, f.st, c->devp, f.goff, f.poff, f.nvec, args...);
+}
 
 BNET_API int bnet_fused_allreduce_sgd(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, float lr,
                                       float momentum, float weight_decay, float grad_scale, float* master,
                                       float* mom_buf, int zero_grads, int channel, int nblocks, void* stream) {
-  return fused_allreduce_sgd_impl(c, grad_off, param_off, count, dtype, lr, momentum, weight_decay, grad_scale, master, mom_buf,
-                                  zero_grads, channel, nblocks, stream, nullptr);
+  FusedLaunch f;
+  if (fused_prologue(c, "SGD", grad_off, param_off, count, dtype, channel, {master, mom_buf}, nblocks, stream, f) < 0) return -1;
+  return run_fused<SgdKernel>(c, dtype, f, lr, momentum, weight_decay, grad_scale, master, mom_buf, zero_grads, channel,
+                              (const float*)nullptr);
 }
 
 // Same, with {lr, momentum, weight_decay, grad_scale} read from 4 floats of device memory at kernel run time.
@@ -1150,57 +1158,19 @@ BNET_API int bnet_fused_allreduce_sgd_hp(BnetColl* c, size_t grad_off, size_t pa
                                          const float* hp_dev, float* master, float* mom_buf, int zero_grads, int channel,
                                          int nblocks, void* stream) {
   if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
-  return fused_allreduce_sgd_impl(c, grad_off, param_off, count, dtype, 0.f, 0.f, 0.f, 1.f, master, mom_buf, zero_grads, channel,
-                                  nblocks, stream, hp_dev);
-}
-
-// Input checks shared by the fused optimizer entry points (`what` names the optimizer in the message).
-static int fused_check(BnetColl* c, const char* what, size_t grad_off, size_t param_off, size_t count, int dtype, int channel) {
-  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
-  if (dtype != BNET_F32 && dtype != BNET_BF16) return fail("fused %s supports f32 and bf16", what);
-  size_t bytes = count * elsize(dtype);
-  if (bytes % (16 * (size_t)c->world) || grad_off % 16 || param_off % 16) return fail("fused %s needs 16-byte aligned offsets and bytes%%(16*world)==0", what);
-  if (grad_off + bytes > c->alloc_bytes - kPadBytes || param_off + bytes > c->alloc_bytes - kPadBytes) return fail("fused %s range outside the heap", what);
-  return 0;
-}
-
-static int fused_allreduce_sgd_impl(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, float lr,
-                                    float momentum, float weight_decay, float grad_scale, float* master, float* mom_buf,
-                                    int zero_grads, int channel, int nblocks, void* stream, const float* hp) {
-  if (fused_check(c, "SGD", grad_off, param_off, count, dtype, channel) < 0) return -1;
-  if (((uintptr_t)master | (uintptr_t)mom_buf) & 15) return fail("optimizer state must be 16-byte aligned");
-  refresh_devp(c);
-  size_t nvec = count * elsize(dtype) / 16;
-  int nb = pick_blocks(c, nvec / c->world, nblocks, prefer_nvls(c) && env_int("FUSED_NVLS", 1) ? BLK_FUSED_NVLS : BLK_P2P);
-  cudaStream_t st = (cudaStream_t)stream;
-  size_t goff = kPadBytes + grad_off, poff = kPadBytes + param_off;
-  if (dtype == BNET_F32) return run_fused<BNET_F32>(c, goff, poff, nvec, lr, momentum, weight_decay, grad_scale, master, mom_buf, zero_grads, channel, nb, st, hp);
-  return run_fused<BNET_BF16>(c, goff, poff, nvec, lr, momentum, weight_decay, grad_scale, master, mom_buf, zero_grads, channel, nb, st, hp);
-}
-
-template <int DT>
-static int run_fused_adamw(BnetColl* c, size_t goff, size_t poff, size_t nvec, const float* hp, float* master, float* m1,
-                           float* m2, int zero, int chan, int nb, cudaStream_t st) {
-  if (c->world == 1)
-    return launch(bnet_fused_adamw_kernel<DT, 0>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
-  if (prefer_nvls(c) && env_int("FUSED_NVLS", 1))
-    return launch(bnet_fused_adamw_kernel<DT, 1>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
-  return launch(bnet_fused_adamw_kernel<DT, 2>, nb, kThreads, st, c->devp, goff, poff, nvec, hp, master, m1, m2, zero, chan);
+  FusedLaunch f;
+  if (fused_prologue(c, "SGD", grad_off, param_off, count, dtype, channel, {master, mom_buf}, nblocks, stream, f) < 0) return -1;
+  return run_fused<SgdKernel>(c, dtype, f, 0.f, 0.f, 0.f, 1.f, master, mom_buf, zero_grads, channel, hp_dev);
 }
 
 BNET_API int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype,
                                         const float* hp_dev, float* master, float* exp_avg, float* exp_avg_sq, int zero_grads,
                                         int channel, int nblocks, void* stream) {
-  if (fused_check(c, "AdamW", grad_off, param_off, count, dtype, channel) < 0) return -1;
   if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
-  if (((uintptr_t)master | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) return fail("optimizer state must be 16-byte aligned");
-  refresh_devp(c);
-  size_t nvec = count * elsize(dtype) / 16;
-  int nb = pick_blocks(c, nvec / c->world, nblocks, prefer_nvls(c) && env_int("FUSED_NVLS", 1) ? BLK_FUSED_NVLS : BLK_P2P);
-  cudaStream_t st = (cudaStream_t)stream;
-  size_t goff = kPadBytes + grad_off, poff = kPadBytes + param_off;
-  if (dtype == BNET_F32) return run_fused_adamw<BNET_F32>(c, goff, poff, nvec, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel, nb, st);
-  return run_fused_adamw<BNET_BF16>(c, goff, poff, nvec, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel, nb, st);
+  FusedLaunch f;
+  if (fused_prologue(c, "AdamW", grad_off, param_off, count, dtype, channel, {master, exp_avg, exp_avg_sq}, nblocks, stream, f) < 0)
+    return -1;
+  return run_fused<AdamWKernel>(c, dtype, f, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel);
 }
 
 BNET_API int bnet_pack_cast(const BnetPackItem* items_dev, int n, void* dst, int src_dtype, int dst_dtype, float scale,

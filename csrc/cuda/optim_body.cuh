@@ -1,9 +1,10 @@
-// Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu).
+// Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu): sgd_update for
+// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel.
 //
-// The update is written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into
-// bnet_fused_adamw_kernel by nvcc and (b) compiled by g++ and checked against a long-double AdamW by
-// csrc/tests/optim_emu_test.cc, without a GPU.  Every product that feeds a sum is an explicit fmaf, so nvcc's
-// contraction and g++'s lack of it cannot make the two builds round differently.
+// The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
+// kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks AdamW against a long-double
+// reference), without a GPU.  Every product that feeds a sum is an explicit fmaf, so nvcc's contraction and g++'s
+// lack of it cannot make the two builds round differently.
 #pragma once
 #include <math.h>
 
@@ -15,6 +16,14 @@
 
 namespace bnet {
 namespace optim {
+
+// One element of torch.optim.SGD with momentum and L2 weight decay (dampening 0, no Nesterov):
+//   d_p = grad*gscale + wd*p;  buf = mu*buf + d_p;  p -= lr*buf
+BNET_OPT_HD void sgd_update(float grad, float& p, float& buf, float lr, float mu, float wd, float gscale) {
+  const float dp = fmaf(wd, p, grad * gscale);
+  buf = fmaf(mu, buf, dp);
+  p = fmaf(-lr, buf, p);
+}
 
 // Hyper-parameter block of the fused AdamW kernel: 8 floats of device memory, 16-byte aligned, read when the kernel
 // runs, so a captured CUDA graph follows a learning-rate schedule and the bias correction without being re-captured.

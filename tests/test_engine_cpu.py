@@ -1,79 +1,17 @@
 """The fused data-parallel engine's HOST logic on the CPU: bucket planning, the flat parameter / gradient views (including
 channels_last filters), the hook-driven launches of the per-bucket "collective + optimizer" step, finish_step, learning-rate
-changes, optimizer state save / load.  The symmetric heap and the fused kernel are replaced by a fake comm whose
-`fused_allreduce_sgd` is the same arithmetic in plain PyTorch (world size 1), and the CUDA stream / event calls by stubs —
-bagua_net_b200/parallel/ddp.py itself runs unmodified.  The device side is covered by the GPU tests (tests/test_gpu.py:
+changes, optimizer state save / load.  The symmetric heap, the fused kernel and the CUDA stream / event calls are replaced
+by the stand-ins of tests/engine_fakes.py.  The device side is covered by the GPU tests (tests/test_gpu.py:
 `test_ddp_engine_*`, `test_fused_sgd_*`)."""
-import contextlib
 import copy
 
 import pytest
 import torch
+from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import small_model as _model
 
 from bagua_net_b200.parallel import ddp as ddp_mod
 from bagua_net_b200.parallel.ddp import BnetDDP, plan_buckets
-
-
-class FakeStream:
-    def wait_event(self, ev):
-        pass
-
-    def wait_stream(self, s):
-        pass
-
-    def synchronize(self):
-        pass
-
-
-class FakeEvent:
-    def record(self, s=None):
-        pass
-
-
-class FakeComm:
-    """What BnetDDP needs from SymmComm, for one rank, in host memory."""
-
-    def __init__(self):
-        self.world, self.rank, self.launches = 1, 0, 0
-        self.calls = []
-
-    def alloc(self, numel, dtype):
-        return torch.zeros(numel, dtype=dtype)
-
-    def all_reduce(self, t, op="sum", **kw):
-        return t
-
-    def fused_allreduce_sgd(self, grad, param, master, mom, lr, momentum, weight_decay, grad_scale=None, zero_grads=True, channel=0,
-                            nblocks=0, stream=None, hp=None):
-        if hp is not None:
-            lr, momentum, weight_decay, scale = (float(v) for v in hp[:4])
-        else:
-            scale = 1.0 / self.world if grad_scale is None else grad_scale
-        g = grad.float() * scale + weight_decay * master          # mean gradient + L2 term on the fp32 master weights
-        mom.mul_(momentum).add_(g)
-        master.sub_(lr * mom)
-        param.copy_(master.to(param.dtype))
-        if zero_grads:
-            grad.zero_()
-        self.launches += 1
-        self.calls.append(grad.numel())
-
-
-@pytest.fixture
-def cpu_engine(monkeypatch):
-    monkeypatch.setattr(torch.cuda, "Stream", lambda *a, **k: FakeStream())
-    monkeypatch.setattr(torch.cuda, "Event", lambda *a, **k: FakeEvent())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: FakeStream())
-    monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
-    monkeypatch.setattr(torch.cuda, "stream", lambda s: contextlib.nullcontext())
-    return monkeypatch
-
-
-def _model(channels_last=True):
-    torch.manual_seed(3)
-    m = torch.nn.Sequential(torch.nn.Conv2d(3, 8, 3, padding=1), torch.nn.ReLU(), torch.nn.Conv2d(8, 8, 3, padding=1), torch.nn.ReLU(),
-                            torch.nn.AdaptiveAvgPool2d(2), torch.nn.Flatten(), torch.nn.Linear(32, 10))
-    return m.to(memory_format=torch.channels_last) if channels_last else m
 
 
 def test_plan_buckets_covers_every_parameter_once():
