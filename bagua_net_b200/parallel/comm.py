@@ -25,6 +25,7 @@ DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 OPS = {"sum": 0, "avg": 1, "max": 2, "min": 3}
 ALGOS = {"auto": 0, "nvls": 1, "p2p": 2, "oneshot": 3, "ll": 0}
 BLOB = 128
+CLIP_ROW = 304          # doubles per bucket in the clipped step's partial rows (BNET_COLL_CLIP_ROW)
 
 
 def _host_identity():
@@ -78,6 +79,11 @@ def _declare(lib):
                                              i, i, i, vp]
     lib.bnet_fused_allreduce_sgd_hp.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, i, i, i, vp]
     lib.bnet_fused_allreduce_adamw.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, vp, i, i, i, vp]
+    lib.bnet_fused_clip_reduce_norm.argtypes = [vp, sz, sz, i, vp, vp, i, i, vp]
+    lib.bnet_fused_clip_coef.argtypes = [vp, vp, i, sz, C.c_float, vp, i, vp]
+    lib.bnet_fused_clip_apply_sgd.argtypes = [vp, sz, sz, i, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp, i, i, vp]
+    lib.bnet_fused_clip_apply_sgd_hp.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, vp, i, i, vp]
+    lib.bnet_fused_clip_apply_adamw.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, vp, vp, i, i, vp]
     lib.bnet_pack_cast.argtypes = [vp, i, vp, i, i, C.c_float, C.c_uint64, vp]
 
 
@@ -267,6 +273,64 @@ class SymmComm:
         n = self._chk(getattr(self.lib, "bnet_" + name)(
             self.h, self.offset_of(grad), self.offset_of(param), grad.numel(), DT[grad.dtype], *scalars,
             *(C.c_void_p(s.data_ptr()) for s in state), 1 if zero_grads else 0, channel, nblocks, self._stream(stream)), name)
+        self.launches += n
+
+    # ------------------------------------------------------------------ fused step with gradient clipping (three stages)
+    def fused_clip_reduce_norm(self, grad: torch.Tensor, scratch: torch.Tensor, partial: torch.Tensor, channel: int = 0,
+                               nblocks: int = 0, stream=None):
+        """Stage 1, per bucket: sum-reduce ``grad`` across ranks into this rank's fp32 ``scratch`` shard (numel/world),
+        write each CTA's sum of squares to its slot of the float64 ``partial`` row (``CLIP_ROW`` slots) and zero ``grad``."""
+        assert scratch.dtype == torch.float32 and scratch.is_contiguous() and scratch.numel() * self.world == grad.numel()
+        assert partial.is_cuda and partial.dtype == torch.float64 and partial.is_contiguous() and partial.numel() >= CLIP_ROW
+        n = self._chk(self.lib.bnet_fused_clip_reduce_norm(
+            self.h, self.offset_of(grad), grad.numel(), DT[grad.dtype], C.c_void_p(scratch.data_ptr()),
+            C.c_void_p(partial.data_ptr()), channel, nblocks, self._stream(stream)), "fused_clip_reduce_norm")
+        self.launches += n
+
+    def fused_clip_coef(self, partials: torch.Tensor, xchg: torch.Tensor, clip: torch.Tensor, grad_scale: float | None = None,
+                        channel: int = 0, stream=None):
+        """Stage 2, once per step: the global norm from every rank's ``partials`` ([buckets, CLIP_ROW] float64), exchanged
+        through the heap tensor ``xchg`` (at least ``world`` float64), times ``grad_scale`` (default 1/world: the norm of
+        the mean gradient); writes total_norm and clip_coef into ``clip`` ({max_norm, total_norm, clip_coef, reserved})."""
+        assert partials.is_cuda and partials.dtype == torch.float64 and partials.is_contiguous()
+        assert partials.dim() == 2 and partials.shape[1] == CLIP_ROW
+        assert xchg.numel() * xchg.element_size() >= 8 * self.world
+        assert clip.is_cuda and clip.dtype == torch.float32 and clip.numel() >= 4 and clip.is_contiguous()
+        gs = (1.0 / self.world) if grad_scale is None else grad_scale
+        n = self._chk(self.lib.bnet_fused_clip_coef(self.h, C.c_void_p(partials.data_ptr()), partials.shape[0],
+                                                    self.offset_of(xchg), gs, C.c_void_p(clip.data_ptr()), channel,
+                                                    self._stream(stream)), "fused_clip_coef")
+        self.launches += n
+
+    def fused_clip_apply_sgd(self, param: torch.Tensor, scratch: torch.Tensor, clip: torch.Tensor, master: torch.Tensor,
+                             mom: torch.Tensor, lr: float, momentum: float, weight_decay: float, grad_scale: float | None = None,
+                             channel: int = 0, nblocks: int = 0, stream=None, hp: torch.Tensor | None = None):
+        """Stage 3, per bucket: the SGD step of ``fused_allreduce_sgd`` from ``scratch`` times clip_coef, and the new
+        ``param`` on every rank."""
+        gs = (1.0 / self.world) if grad_scale is None else grad_scale
+        self._clip_apply("fused_clip_apply_sgd" if hp is None else "fused_clip_apply_sgd_hp", param, scratch, clip,
+                         (master, mom), (lr, momentum, weight_decay, gs), hp, 4, channel, nblocks, stream)
+
+    def fused_clip_apply_adamw(self, param: torch.Tensor, scratch: torch.Tensor, clip: torch.Tensor, master: torch.Tensor,
+                               exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, hp: torch.Tensor, channel: int = 0,
+                               nblocks: int = 0, stream=None):
+        """Stage 3, per bucket: the AdamW step of ``fused_allreduce_adamw`` from ``scratch`` times clip_coef, and the new
+        ``param`` on every rank."""
+        assert hp is not None
+        self._clip_apply("fused_clip_apply_adamw", param, scratch, clip, (master, exp_avg, exp_avg_sq), (), hp, 8, channel,
+                         nblocks, stream)
+
+    def _clip_apply(self, name, param, scratch, clip, state, scalars, hp, hp_words, channel, nblocks, stream):
+        assert scratch.dtype == torch.float32 and scratch.is_contiguous() and scratch.numel() * self.world == param.numel()
+        assert clip.is_cuda and clip.dtype == torch.float32 and clip.numel() >= 4 and clip.is_contiguous()
+        assert all(s.dtype == torch.float32 and s.numel() * self.world == param.numel() for s in state)
+        if hp is not None:
+            assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= hp_words and hp.is_contiguous()
+            scalars = (C.c_void_p(hp.data_ptr()),)
+        n = self._chk(getattr(self.lib, "bnet_" + name)(
+            self.h, self.offset_of(param), param.numel(), DT[param.dtype], C.c_void_p(scratch.data_ptr()),
+            C.c_void_p(clip.data_ptr()), *scalars, *(C.c_void_p(s.data_ptr()) for s in state), channel, nblocks,
+            self._stream(stream)), name)
         self.launches += n
 
     # ------------------------------------------------------------------ collectives on ordinary tensors

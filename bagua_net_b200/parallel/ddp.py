@@ -136,14 +136,24 @@ def direct_grads_self_check(device=None, group=None, steps: int = 3, make_model=
 _STATE_NAMES = {"sgd": ("master", "momentum"), "adamw": ("master", "exp_avg", "exp_avg_sq")}
 
 
+def _check_max_norm(v) -> float:
+    v = float(v)
+    if not v > 0.0:                       # (False for NaN as well)
+        raise ValueError(f"max_grad_norm must be > 0 or inf (got {v}); only the L2 norm is offered")
+    return v
+
+
 class _Bucket:
-    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state")
+    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state", "scratch", "partial", "launched")
 
     def __init__(self):
         self.params = []
         self.start = 0
         self.numel = 0
         self.ready = 0
+        self.scratch = None          # clipped step: this rank's fp32 shard of the rank-summed gradient
+        self.partial = None          # clipped step: the bucket's row of per-CTA sums of squares
+        self.launched = False        # clipped step: stage 1 ran for this bucket in the current step
 
     @property
     def master(self) -> torch.Tensor:
@@ -156,13 +166,20 @@ class BnetDDP(torch.nn.Module):
     AMSGrad and ``maximize`` are not offered).
 
     bucket_mb sizes buckets for launch latency and overlap (NVSwitch: no per-link bound).
+
+    max_grad_norm: clip the mean gradient by its global L2 norm before the update, as
+    ``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)`` does (``inf`` computes the norm and never clips).  The step
+    then runs in three stages: per bucket from the gradient hook, reduce into an fp32 scratch and sum squares; once per
+    step, the norm and the coefficient; per bucket, the update from the scratch.  ``None`` keeps the one-kernel step.
     """
 
     def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float | None = None, weight_decay: float = 0.0,
                  bucket_mb: float = 64.0, comm: SymmComm | None = None, extra_heap_bytes: int = 64 << 20,
                  nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
-                 eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False):
+                 eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None):
         super().__init__()
+        if max_grad_norm is not None:
+            max_grad_norm = _check_max_norm(max_grad_norm)
         if optimizer not in ("sgd", "adamw"):
             raise ValueError(f"unknown optimizer {optimizer!r}: BnetDDP fuses 'sgd' or 'adamw'")
         if amsgrad or maximize:
@@ -272,6 +289,18 @@ class BnetDDP(torch.nn.Module):
         # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh); SGD
         # passes them as launch arguments until the first set_lr
         self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev) if optimizer == "adamw" else None
+        # gradient clipping: per bucket an fp32 scratch shard and a row of per-CTA partial sums of squares, one exchange
+        # area in the heap (same offset on every rank) and the device block {max_norm, total_norm, clip_coef, reserved}
+        self._clip = None
+        if max_grad_norm is not None:
+            from .comm import CLIP_ROW
+
+            self._partials = torch.zeros(len(self.buckets), CLIP_ROW, dtype=torch.float64, device=dev)
+            for b, row in zip(self.buckets, self._partials):
+                b.scratch, b.partial = torch.zeros_like(b.master), row
+            self._xchg = comm.alloc(comm.world, torch.float64)
+            self._clip = torch.tensor([max_grad_norm, 0.0, 0.0, 0.0], dtype=torch.float32, device=dev)
+        self.max_grad_norm = max_grad_norm
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad) for p in params]
@@ -300,7 +329,11 @@ class BnetDDP(torch.nn.Module):
         ev = torch.cuda.Event()
         ev.record(cur)
         self.comm_stream.wait_event(ev)          # the bucket's gradients are complete on the compute stream
-        if self.optimizer == "adamw":
+        if self._clip is not None:               # clipped step, stage 1: reduce into the scratch, sum of squares
+            self.comm.fused_clip_reduce_norm(b.grad, b.scratch, b.partial, channel=0, nblocks=self.nblocks,
+                                             stream=self.comm_stream)
+            b.launched = True
+        elif self.optimizer == "adamw":
             self.comm.fused_allreduce_adamw(b.grad, b.param, *b.state, self._hp, zero_grads=True, channel=0,
                                             nblocks=self.nblocks, stream=self.comm_stream)
         else:
@@ -316,6 +349,8 @@ class BnetDDP(torch.nn.Module):
             if b.ready:                           # parameters that got no gradient this step
                 self._launch(b)
         if self._inflight:
+            if self._clip is not None:
+                self._clipped_update()
             if self.optimizer == "adamw":
                 # one optimizer step taken: advance the step count the kernels read, behind this step's last bucket
                 # (on the comm stream, so a captured step replays it)
@@ -323,6 +358,28 @@ class BnetDDP(torch.nn.Module):
                     self._hp[self._HP_STEP:self._HP_STEP + 1].add_(1.0)
             torch.cuda.current_stream().wait_stream(self.comm_stream)
             self._inflight = False
+
+    def _clipped_update(self):
+        """Stages 2 and 3 of the clipped step, on the comm stream behind every bucket's stage 1."""
+        # Behind the whole backward: stage 2's rank barrier then also means that every rank's backward is done, which
+        # is what lets stage 3 write new parameters into the peers without an opening barrier of its own.
+        self.comm_stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.comm_stream):
+            for b in self.buckets:
+                if not b.launched:                # no gradient at all this step: no update, and nothing in the norm
+                    b.partial.zero_()
+        self.comm.fused_clip_coef(self._partials, self._xchg, self._clip, channel=0, stream=self.comm_stream)
+        for b in self.buckets:
+            if not b.launched:
+                continue
+            if self.optimizer == "adamw":
+                self.comm.fused_clip_apply_adamw(b.param, b.scratch, self._clip, *b.state, self._hp, channel=0,
+                                                 nblocks=self.nblocks, stream=self.comm_stream)
+            else:
+                self.comm.fused_clip_apply_sgd(b.param, b.scratch, self._clip, *b.state, self.lr, self.momentum,
+                                               self.weight_decay, channel=0, nblocks=self.nblocks, stream=self.comm_stream,
+                                               hp=self._hp)
+            b.launched = False
 
     # ------------------------------------------------------------------ user API
     def forward(self, *args, **kwargs):
@@ -359,8 +416,7 @@ class BnetDDP(torch.nn.Module):
             # have it; checkpoint/resume stays step-exact.
             live = [self.flat_param] + [t for b in self.buckets for t in b.state]
             live += [t for t in self.module.buffers() if t.is_cuda and t.numel()]
-            if self._hp is not None:
-                live.append(self._hp)
+            live += [t for t in (self._hp, self._clip) if t is not None]
             saved = [t.clone() for t in live]
             for _ in range(2):
                 self._eager_step(self._gx, self._gy, loss_fn)
@@ -560,6 +616,21 @@ class BnetDDP(torch.nn.Module):
             self._graph = None
         else:
             self._hp.copy_(torch.tensor(vals, dtype=torch.float32), non_blocking=False)
+
+    def set_max_grad_norm(self, max_norm: float) -> None:
+        """Change the clipping threshold of an engine built with ``max_grad_norm``.  The norm kernel reads it from
+        device memory, so a captured CUDA graph follows it without being re-captured."""
+        if self._clip is None:
+            raise ValueError("gradient clipping is off: build the engine with max_grad_norm=... to enable it")
+        self.max_grad_norm = _check_max_norm(max_norm)
+        self._clip[:1].copy_(torch.tensor([self.max_grad_norm], dtype=torch.float32))
+
+    @property
+    def last_grad_norm(self) -> torch.Tensor | None:
+        """The global L2 norm of the mean gradient before clipping in the most recent step (what ``clip_grad_norm_``
+        returns), as a new 0-dim fp32 tensor on the device: a copy taken on the current stream, so tensors kept from
+        earlier steps keep their values and reading one is the only synchronisation.  ``None`` without clipping."""
+        return None if self._clip is None else self._clip[1].clone()
 
     # AdamW's hyper-parameter block: {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved}
     _HP_STEP = 6

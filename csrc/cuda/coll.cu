@@ -22,6 +22,7 @@
 
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "bnet/bnet_coll.h"
@@ -495,21 +496,41 @@ struct AdamWOpt {
   }
 };
 
-// One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch reductions / peer loads, the
-// fp32 state) are issued before any dependent math so that U*(1 + S*E/4) requests per thread are in flight: the
-// kernel is latency*bandwidth bound (NVLink round trip ~3 us, HBM), not ALU bound.
-template <int DT, int MODE, int U, class Opt>
-__device__ __forceinline__ void fused_batch(const CollDev& d, size_t goff, size_t poff, size_t start, size_t i, size_t stride,
+// Where the fused step takes the rank-summed gradient from.  HeapGrad: the bucket's gradients at heap byte offset `off`,
+// reduced over the ranks on the fly (fused_grad_issue / fused_grad_get).  ScratchGrad: this rank's shard of them,
+// already reduced into local fp32 memory by bnet_clip_norm_kernel (the same floats fused_grad_get would give), times
+// the clipping coefficient.
+struct HeapGrad {
+  size_t off;
+};
+struct ScratchGrad {
+  const float* g;
+  float coef;
+};
+
+// One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch reductions / peer loads or the
+// fp32 scratch, the fp32 state) are issued before any dependent math so that U*(1 + S*E/4) requests per thread are in
+// flight: the kernel is latency*bandwidth bound (NVLink round trip ~3 us, HBM), not ALU bound.
+template <int DT, int MODE, int U, class Opt, class G>
+__device__ __forceinline__ void fused_batch(const CollDev& d, const G& src, size_t poff, size_t start, size_t i, size_t stride,
                                             const Opt& opt, float* const (&state)[Opt::kStates]) {
   constexpr int E = VecTraits<DT>::kElems;
   constexpr int Q = E / 4;
   constexpr int S = Opt::kStates;
+  constexpr bool kHeap = std::is_same<G, HeapGrad>::value;
   int4 gv[U];
   float4 sm[U][S][Q];
   float gp2p[(MODE == 2) ? U : 1][8];
+  float4 gs[kHeap ? 1 : U][Q];
 #pragma unroll
-  for (int u = 0; u < U; u++)
-    fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
+  for (int u = 0; u < U; u++) {
+    if constexpr (kHeap) {
+      fused_grad_issue<DT, MODE>(d, src.off + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
+    } else {
+#pragma unroll
+      for (int q = 0; q < Q; q++) gs[u][q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(src.g + (i + u * stride) * E) + q);
+    }
+  }
 #pragma unroll
   for (int u = 0; u < U; u++)
 #pragma unroll
@@ -519,7 +540,15 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, size_t goff, size_
 #pragma unroll
   for (int u = 0; u < U; u++) {
     float g[8], st[S][8];
-    fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
+    if constexpr (kHeap) {
+      fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
+    } else {
+#pragma unroll
+      for (int q = 0; q < Q; q++) {
+        g[4 * q] = gs[u][q].x * src.coef; g[4 * q + 1] = gs[u][q].y * src.coef;
+        g[4 * q + 2] = gs[u][q].z * src.coef; g[4 * q + 3] = gs[u][q].w * src.coef;
+      }
+    }
 #pragma unroll
     for (int q = 0; q < Q; q++)
 #pragma unroll
@@ -538,21 +567,28 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, size_t goff, size_
   }
 }
 
-// barrier, reduce + update + broadcast of this rank's shard, barrier, gradient zeroing
-template <int DT, int MODE, class Opt>
-__device__ __forceinline__ void fused_step(const CollDev& d, size_t goff, size_t poff, size_t nvec, const Opt& opt,
+// barrier, reduce + update + broadcast of this rank's shard, barrier, gradient zeroing.
+// From the scratch (the clipped step's apply stage) there is neither the opening barrier nor the zeroing.  The opening
+// barrier guards two things: every rank's gradients of the bucket are complete before peers read them, and no rank
+// still reads its parameters (backward) when the new ones arrive.  The apply stage reads no peer's gradients, and it
+// runs behind bnet_clip_coef_kernel, whose rank barrier every rank reaches only after its comm stream waited for its
+// whole backward.  The gradients were zeroed by the norm stage.
+template <int DT, int MODE, class Opt, class G>
+__device__ __forceinline__ void fused_step(const CollDev& d, const G& src, size_t poff, size_t nvec, const Opt& opt,
                                            float* const (&state)[Opt::kStates], int zero_grads, int chan) {
-  if constexpr (MODE != 0) rank_barrier(d, chan);
+  constexpr bool kHeap = std::is_same<G, HeapGrad>::value;
+  if constexpr (MODE != 0 && kHeap) rank_barrier(d, chan);
   const size_t per = nvec / d.world;
   const size_t start = (size_t)d.rank * per;
   const size_t stride = (size_t)gridDim.x * kThreads;
   constexpr int U = Opt::kU;
   size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  for (; i + (U - 1) * stride < per; i += U * stride) fused_batch<DT, MODE, U>(d, goff, poff, start, i, stride, opt, state);
+  for (; i + (U - 1) * stride < per; i += U * stride) fused_batch<DT, MODE, U>(d, src, poff, start, i, stride, opt, state);
   if constexpr (U > 1)
-    for (; i < per; i += stride) fused_batch<DT, MODE, 1>(d, goff, poff, start, i, stride, opt, state);
+    for (; i < per; i += stride) fused_batch<DT, MODE, 1>(d, src, poff, start, i, stride, opt, state);
   if constexpr (MODE != 0) rank_barrier(d, chan);
-  if (zero_grads) fused_zero_grads(d, goff, nvec, per, stride);
+  if constexpr (kHeap)
+    if (zero_grads) fused_zero_grads(d, src.off, nvec, per, stride);
 }
 
 template <int DT, int MODE>
@@ -569,7 +605,7 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_fused_sgd_kernel(CollDev d, 
     gscale = hp[3];
   }
   float* const state[2] = {master, mom};
-  fused_step<DT, MODE>(d, goff, poff, nvec, SgdOpt{lr, mu, wd, gscale}, state, zero_grads, chan);
+  fused_step<DT, MODE>(d, HeapGrad{goff}, poff, nvec, SgdOpt{lr, mu, wd, gscale}, state, zero_grads, chan);
 }
 
 // hp: the 8-float block of optim_body.cuh, always read from device memory.
@@ -579,7 +615,124 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_fused_adamw_kernel(CollDev d
                                                                    float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                                    int zero_grads, int chan) {
   float* const state[3] = {master, exp_avg, exp_avg_sq};
-  fused_step<DT, MODE>(d, goff, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, zero_grads, chan);
+  fused_step<DT, MODE>(d, HeapGrad{goff}, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, zero_grads, chan);
+}
+
+// ------------------------------------------------------------------ gradient clipping by global norm (three stages)
+// Sum of one double per thread of a kThreads-thread CTA in a fixed order (a butterfly inside each warp, then the warps
+// in order), so the same inputs give the same bits.  The sum is valid in thread 0.  One call per kernel.
+__device__ __forceinline__ double cta_sum(double v) {
+  __shared__ double warp_sums[kThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kThreads / 32; w++) s += warp_sums[w];
+  return s;
+}
+
+// Stage 1, one launch per bucket from the gradient hook: barrier, reduce this rank's shard (the one-kernel path's
+// fused_grad_issue / fused_grad_get), store the rank-summed gradient as fp32 into the local `scratch` shard, barrier,
+// zero the gradients (the CTA-paired rule of fused_zero_grads).  Each CTA writes the sum of squares of what it stored
+// to its own slot of the bucket's `partial` row (BNET_COLL_MAX_BLOCKS doubles; CTA 0 zeroes the slots beyond the
+// grid).  No atomics: the same grid gives the same bits.  Squares and sums are taken in double: a square of an fp32
+// value is exact there, and a sum of n of them is within n * 2^-53 of the exact one.
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_norm_kernel(CollDev d, size_t goff, size_t nvec, float* __restrict__ scratch,
+                                                                 double* __restrict__ partial, int chan) {
+  constexpr int E = VecTraits<DT>::kElems;
+  constexpr int Q = E / 4;
+  constexpr int U = 2;
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  const size_t per = nvec / d.world;
+  const size_t start = (size_t)d.rank * per;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  double acc = 0.0;
+  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < per; i += U * stride) {
+    int4 gv[U];
+    float gp2p[(MODE == 2) ? U : 1][8];
+#pragma unroll
+    for (int u = 0; u < U; u++)
+      if (i + u * stride < per) fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      if (i + u * stride >= per) continue;
+      float g[8];
+      fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
+#pragma unroll
+      for (int q = 0; q < Q; q++)
+        ptx::st_na_f4(reinterpret_cast<float4*>(scratch + (i + u * stride) * E) + q,
+                      make_float4(g[4 * q], g[4 * q + 1], g[4 * q + 2], g[4 * q + 3]));
+#pragma unroll
+      for (int k = 0; k < E; k++) acc = fma((double)g[k], (double)g[k], acc);
+    }
+  }
+  acc = cta_sum(acc);
+  if (threadIdx.x == 0) partial[blockIdx.x] = acc;
+  if (blockIdx.x == 0)
+    for (int j = gridDim.x + threadIdx.x; j < BNET_COLL_MAX_BLOCKS; j += kThreads) partial[j] = 0.0;
+  if constexpr (MODE != 0) rank_barrier(d, chan);
+  fused_zero_grads(d, goff, nvec, per, stride);
+}
+
+// Stage 2, one CTA per step after the last bucket's stage 1: sum this rank's `n` partials (all its rows) in a fixed
+// order, exchange the per-rank sums through `world` doubles at heap byte offset `xoff`, add them in rank order
+// 0..world-1 (every rank gets the same bits), and write total_norm = sqrt(sum) * gscale and clip_coef into the clip
+// block.  The exchange slots are reused every step: the second rank barrier is passed only once every rank has read
+// its slots, so no rank's next write can overtake a peer's read.
+__global__ void __launch_bounds__(kThreads) bnet_clip_coef_kernel(CollDev d, const double* __restrict__ partials, size_t n,
+                                                                 size_t xoff, float gscale, float* __restrict__ clip, int chan) {
+  double s = 0.0;
+  for (size_t j = threadIdx.x; j < n; j += kThreads) s += partials[j];
+  s = cta_sum(s);
+  if (d.world > 1) {
+    if (threadIdx.x == 0)
+      for (int p = 0; p < d.world; p++) reinterpret_cast<volatile double*>(d.heap[p] + xoff)[d.rank] = s;
+    rank_barrier(d, chan);
+    if (threadIdx.x == 0) {
+      const volatile double* x = reinterpret_cast<const volatile double*>(d.heap[d.rank] + xoff);
+      s = x[0];
+      for (int q = 1; q < d.world; q++) s += x[q];
+    }
+    rank_barrier(d, chan);
+  }
+  if (threadIdx.x == 0) {
+    const float total = (float)(sqrt(s) * (double)gscale);
+    clip[optim::kClipTotalNorm] = total;
+    clip[optim::kClipCoef] = optim::clip_coef(clip[optim::kClipMaxNorm], total);
+  }
+}
+
+// Stage 3, one launch per bucket after stage 2: the optimizer step of fused_step from the fp32 scratch times clip_coef,
+// then the parameter broadcast and the closing barrier.  Same hyper-parameters as bnet_fused_sgd_kernel /
+// bnet_fused_adamw_kernel.
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_sgd_kernel(CollDev d, size_t poff, size_t nvec,
+                                                                      const float* __restrict__ scratch, const float* __restrict__ clip,
+                                                                      float lr, float mu, float wd, float gscale,
+                                                                      float* __restrict__ master, float* __restrict__ mom, int chan,
+                                                                      const float* __restrict__ hp) {
+  if (hp != nullptr) {
+    lr = hp[0];
+    mu = hp[1];
+    wd = hp[2];
+    gscale = hp[3];
+  }
+  float* const state[2] = {master, mom};
+  fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec, SgdOpt{lr, mu, wd, gscale}, state, 0, chan);
+}
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_adamw_kernel(CollDev d, size_t poff, size_t nvec,
+                                                                        const float* __restrict__ scratch, const float* __restrict__ clip,
+                                                                        const float* __restrict__ hp, float* __restrict__ master,
+                                                                        float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+                                                                        int chan) {
+  float* const state[3] = {master, exp_avg, exp_avg_sq};
+  fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, 0,
+                       chan);
 }
 
 // ------------------------------------------------------------------ multi-tensor pack + cast (K5)
@@ -1134,14 +1287,20 @@ static int fused_prologue(BnetColl* c, const char* what, size_t grad_off, size_t
   return 0;
 }
 
-// Launches K's kernel for `dtype` in MODE 0 on one GPU, 1 with NVLS, 2 with peer loads and stores.
+// Launches K's kernel for `dtype` in MODE 0 on one GPU, 1 with NVLS, 2 with peer loads and stores, with `args` after
+// the communicator.
 template <class K, typename... A>
-static int run_fused(BnetColl* c, int dtype, const FusedLaunch& f, A... args) {
+static int run_fused_kernel(BnetColl* c, int dtype, const FusedLaunch& f, A... args) {
   const int mode = c->world == 1 ? 0 : f.nvls ? 1 : 2;
   const std::decay_t<decltype(K::template fn<BNET_F32, 0>)> kern[2][3] = {
       {K::template fn<BNET_F32, 0>, K::template fn<BNET_F32, 1>, K::template fn<BNET_F32, 2>},
       {K::template fn<BNET_BF16, 0>, K::template fn<BNET_BF16, 1>, K::template fn<BNET_BF16, 2>}};
-  return launch(kern[dtype == BNET_BF16][mode], f.nb, kThreads, f.st, c->devp, f.goff, f.poff, f.nvec, args...);
+  return launch(kern[dtype == BNET_BF16][mode], f.nb, kThreads, f.st, c->devp, args...);
+}
+// The one-kernel steps: gradient and parameter offsets and the vector count first.
+template <class K, typename... A>
+static int run_fused(BnetColl* c, int dtype, const FusedLaunch& f, A... args) {
+  return run_fused_kernel<K>(c, dtype, f, f.goff, f.poff, f.nvec, args...);
 }
 
 BNET_API int bnet_fused_allreduce_sgd(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, float lr,
@@ -1171,6 +1330,77 @@ BNET_API int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t par
   if (fused_prologue(c, "AdamW", grad_off, param_off, count, dtype, channel, {master, exp_avg, exp_avg_sq}, nblocks, stream, f) < 0)
     return -1;
   return run_fused<AdamWKernel>(c, dtype, f, hp_dev, master, exp_avg, exp_avg_sq, zero_grads, channel);
+}
+
+// ---- gradient clipping by global norm: the three stages of the clipped step
+struct ClipNormKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_clip_norm_kernel<DT, MODE>;
+};
+struct ClipSgdKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_clip_apply_sgd_kernel<DT, MODE>;
+};
+struct ClipAdamWKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_clip_apply_adamw_kernel<DT, MODE>;
+};
+
+static int clip_block_check(const float* clip) {
+  if (!clip || ((uintptr_t)clip & 15)) return fail("clip block must be a 16-byte aligned device pointer");
+  return 0;
+}
+
+BNET_API int bnet_fused_clip_reduce_norm(BnetColl* c, size_t grad_off, size_t count, int dtype, float* scratch, double* partial,
+                                         int channel, int nblocks, void* stream) {
+  if (!partial || ((uintptr_t)partial & 7)) return fail("partial row must be an 8-byte aligned device pointer");
+  FusedLaunch f;
+  if (fused_prologue(c, "clip norm", grad_off, grad_off, count, dtype, channel, {scratch}, nblocks, stream, f) < 0) return -1;
+  return run_fused_kernel<ClipNormKernel>(c, dtype, f, f.goff, f.nvec, scratch, partial, channel);
+}
+
+BNET_API int bnet_fused_clip_coef(BnetColl* c, const double* partials, int nrows, size_t xchg_off, float grad_scale, float* clip,
+                                  int channel, void* stream) {
+  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
+  if (nrows < 1 || !partials || ((uintptr_t)partials & 7)) return fail("clip coefficient needs >= 1 partial row, 8-byte aligned");
+  if (clip_block_check(clip) < 0) return -1;
+  if (xchg_off % 16 || xchg_off + (size_t)c->world * sizeof(double) > c->alloc_bytes - kPadBytes)
+    return fail("clip exchange area must be 16-byte aligned and inside the heap");
+  refresh_devp(c);
+  return launch(bnet_clip_coef_kernel, 1, kThreads, (cudaStream_t)stream, c->devp, partials,
+                (size_t)nrows * BNET_COLL_MAX_BLOCKS, kPadBytes + xchg_off, grad_scale, clip, channel);
+}
+
+BNET_API int bnet_fused_clip_apply_sgd(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                       const float* clip, float lr, float momentum, float weight_decay, float grad_scale,
+                                       float* master, float* mom_buf, int channel, int nblocks, void* stream) {
+  if (clip_block_check(clip) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "clipped SGD", param_off, param_off, count, dtype, channel, {scratch, master, mom_buf}, nblocks, stream, f) < 0)
+    return -1;
+  return run_fused_kernel<ClipSgdKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, lr, momentum, weight_decay, grad_scale, master,
+                                         mom_buf, channel, (const float*)nullptr);
+}
+
+BNET_API int bnet_fused_clip_apply_sgd_hp(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                          const float* clip, const float* hp_dev, float* master, float* mom_buf, int channel,
+                                          int nblocks, void* stream) {
+  if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (clip_block_check(clip) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "clipped SGD", param_off, param_off, count, dtype, channel, {scratch, master, mom_buf}, nblocks, stream, f) < 0)
+    return -1;
+  return run_fused_kernel<ClipSgdKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, 0.f, 0.f, 0.f, 1.f, master, mom_buf, channel,
+                                         hp_dev);
+}
+
+BNET_API int bnet_fused_clip_apply_adamw(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                         const float* clip, const float* hp_dev, float* master, float* exp_avg, float* exp_avg_sq,
+                                         int channel, int nblocks, void* stream) {
+  if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (clip_block_check(clip) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "clipped AdamW", param_off, param_off, count, dtype, channel, {scratch, master, exp_avg, exp_avg_sq}, nblocks,
+                     stream, f) < 0)
+    return -1;
+  return run_fused_kernel<ClipAdamWKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, hp_dev, master, exp_avg, exp_avg_sq, channel);
 }
 
 BNET_API int bnet_pack_cast(const BnetPackItem* items_dev, int n, void* dst, int src_dtype, int dst_dtype, float scale,

@@ -1,5 +1,5 @@
 // Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu): sgd_update for
-// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel.
+// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, and clip_coef for the clipped step.
 //
 // The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
 // kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks AdamW against a long-double
@@ -71,6 +71,20 @@ BNET_OPT_HD void adamw_update(float grad, float& p, float& m, float& v, const Ad
   const float denom = sqrtf(v) / c.bc2_sqrt + c.eps;
   p = fmaf(-c.step_size, m / denom, p);
 }
+
+// Gradient clipping by global norm, as torch.nn.utils.clip_grad_norm_(norm_type=2, error_if_nonfinite=False):
+//   clip_coef = clamp(max_norm / (total_norm + 1e-6), max=1)
+// in fp32, like torch's fp32 norm tensor.  clamp propagates NaN and fminf(1, NaN) does not, so the clamp is a compare
+// that is false for NaN: a NaN norm gives a NaN coefficient.  An infinite norm gives 0 (and an infinite gradient
+// element times 0 gives NaN), max_norm = inf with a finite norm gives 1.
+BNET_OPT_HD float clip_coef(float max_norm, float total_norm) {
+  const float c = max_norm / (total_norm + 1e-6f);
+  return c > 1.0f ? 1.0f : c;
+}
+
+// Device block of the clipped step (separate from the optimizers' hyper-parameter blocks): 4 floats, 16-byte aligned.
+// max_norm is written by the host; the norm kernel writes total_norm (before clipping) and clip_coef every step.
+enum { kClipMaxNorm = 0, kClipTotalNorm, kClipCoef, kClipReserved, kClipWords };
 
 }  // namespace optim
 }  // namespace bnet

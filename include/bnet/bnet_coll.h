@@ -97,6 +97,38 @@ int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t param_off, s
                                float* master, float* exp_avg, float* exp_avg_sq, int zero_grads, int channel, int nblocks,
                                void* stream);
 
+/* Fused step with gradient clipping by global L2 norm (torch.nn.utils.clip_grad_norm_, norm type 2), in three stages on
+ * one stream.  The clip block is 4 floats of device memory, 16-byte aligned: {max_norm, total_norm, clip_coef, reserved};
+ * the caller writes max_norm, stage 2 writes the other two every step.
+ *
+ * Stage 1, per bucket: reduce the bucket's gradients over the ranks like bnet_fused_allreduce_sgd, but store this rank's
+ * shard of the sum as fp32 in `scratch` (count/world floats, 16-byte aligned) instead of updating, write the sum of squares
+ * of each CTA's share (in double) to its slot of the `partial` row (BNET_COLL_CLIP_ROW doubles; slots beyond the grid are
+ * zeroed), and zero grad[bucket].  Deterministic: no atomics, the same grid gives the same bits. */
+#define BNET_COLL_CLIP_ROW BNET_COLL_MAX_BLOCKS
+int bnet_fused_clip_reduce_norm(BnetColl* c, size_t grad_off, size_t count, int dtype, float* scratch, double* partial,
+                                int channel, int nblocks, void* stream);
+/* Stage 2, once per step after every bucket's stage 1 (and after the caller's stream has waited for backward): sum the
+ * nrows x BNET_COLL_CLIP_ROW doubles at `partials` in a fixed order, exchange the per-rank sums through `world` doubles at
+ * heap byte offset `xchg_off` (16-byte aligned, same offset on every rank, used by nothing else) and add them in rank
+ * order, so every rank gets the same bits; then total_norm = sqrt(sum) * grad_scale and
+ * clip_coef = clamp(max_norm / (total_norm + 1e-6), max=1) (NaN propagates).  One CTA, two rank barriers. */
+int bnet_fused_clip_coef(BnetColl* c, const double* partials, int nrows, size_t xchg_off, float grad_scale, float* clip,
+                         int channel, void* stream);
+/* Stage 3, per bucket after stage 2: the SGD or AdamW update of bnet_fused_allreduce_sgd[_hp] / _adamw with the gradient
+ * scratch[i] * clip_coef in place of the rank-summed gradient, then the parameter broadcast and a closing barrier.  No
+ * gradient zeroing (stage 1 did it).  With max_norm = inf and a finite norm, clip_coef is 1 and the result is bitwise the
+ * one-kernel step's. */
+int bnet_fused_clip_apply_sgd(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch, const float* clip,
+                              float lr, float momentum, float weight_decay, float grad_scale, float* master, float* mom_buf,
+                              int channel, int nblocks, void* stream);
+int bnet_fused_clip_apply_sgd_hp(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                 const float* clip, const float* hp_dev, float* master, float* mom_buf, int channel, int nblocks,
+                                 void* stream);
+int bnet_fused_clip_apply_adamw(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch, const float* clip,
+                                const float* hp_dev, float* master, float* exp_avg, float* exp_avg_sq, int channel, int nblocks,
+                                void* stream);
+
 /* Multi-tensor pack+cast into the heap (K5): n tensors described on the device. */
 typedef struct {
   const void* src;
