@@ -86,7 +86,7 @@ $(BUILD)/tests/exec_emu_test: csrc/tests/exec_emu_test.cc csrc/cuda/exec_body.cu
 $(BUILD)/tests/tc_emu_test: csrc/tests/tc_emu_test.cc csrc/cuda/tc_body.cuh include/bnet/bnet_tc.h
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) -Iinclude $< -o $@
-# the fused AdamW kernel's per-element update against a long-double AdamW
+# the fused SGD and AdamW kernels' per-element updates against long-double SGD and AdamW
 $(BUILD)/tests/optim_emu_test: csrc/tests/optim_emu_test.cc csrc/cuda/optim_body.cuh
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) $< -o $@

@@ -2,8 +2,8 @@
 // bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, and clip_coef for the clipped step.
 //
 // The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
-// kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks AdamW against a long-double
-// reference), without a GPU.  Every product that feeds a sum is an explicit fmaf, so nvcc's contraction and g++'s
+// kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks SGD and AdamW against long-double
+// references), without a GPU.  Every product that feeds a sum is an explicit fmaf, so nvcc's contraction and g++'s
 // lack of it cannot make the two builds round differently.
 #pragma once
 #include <math.h>
@@ -19,9 +19,14 @@ namespace optim {
 
 // One element of torch.optim.SGD with momentum and L2 weight decay (dampening 0, no Nesterov):
 //   d_p = grad*gscale + wd*p;  buf = mu*buf + d_p;  p -= lr*buf
+// torch skips the terms of a zero hyper-parameter: with wd == 0 it does not read p, and with mu == 0 it keeps no
+// buffer and steps with d_p alone.  So does this: once an infinite gradient has made p or buf infinite, 0 * inf would
+// turn every later step of the element into NaN where torch keeps the infinity.  With mu == 0, buf = d_p is still
+// stored, so the state layout does not depend on mu.  For finite values the selects change nothing: 0 * x + y == y.
 BNET_OPT_HD void sgd_update(float grad, float& p, float& buf, float lr, float mu, float wd, float gscale) {
-  const float dp = fmaf(wd, p, grad * gscale);
-  buf = fmaf(mu, buf, dp);
+  const float g = grad * gscale;
+  const float dp = wd == 0.0f ? g : fmaf(wd, p, g);
+  buf = mu == 0.0f ? dp : fmaf(mu, buf, dp);
   p = fmaf(-lr, buf, p);
 }
 

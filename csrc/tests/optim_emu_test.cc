@@ -1,7 +1,8 @@
-// CPU test of the fused AdamW update: compiles the per-element body of csrc/cuda/optim_body.cuh (what
-// bnet_fused_adamw_kernel inlines) with g++ and compares it with a long-double AdamW fed the same fp32 inputs and
-// the same fp32 hyper-parameters.
+// CPU test of the fused optimizer updates: compiles the per-element bodies of csrc/cuda/optim_body.cuh (what
+// bnet_fused_adamw_kernel and bnet_fused_sgd_kernel inline) with g++ and compares them with a long-double AdamW and SGD
+// fed the same fp32 inputs and the same fp32 hyper-parameters.  The SGD part and its bound are further down.
 //
+// AdamW:
 // Bound (u = 2^-24, F = 4 * 2^-149 for results in the subnormal range).  With M = b1|m| + (1-b1)|g|,
 // V = b2 v + (1-b2) g^2, S = lr / (1 - b1^t), D the reference denominator and m1, p2 the reference results:
 //   |m - m1| <= 4u M + F,   |v - v1| <= 6u V + F,
@@ -76,7 +77,7 @@ static void check_one(const Hp& h, float g, float p, float m, float v, const cha
   }
 }
 
-int main() {
+static void adamw_checks() {
   const float steps[] = {0.f, 1.f, 9.f, 99999.f};   // words of the hp block: t = 1, 2, 10, 10^5
   const Hp bases[] = {
       {1e-3f, 0.9f, 0.999f, 1e-8f, 0.f, 1.f, 0},      // torch defaults, Adam (no decay)
@@ -125,7 +126,124 @@ int main() {
       CHECK(isnan(m[k]) == (k == 1) && isnan(v[k]) == (k == 1), "element %d: m=%g v=%g", k, m[k], v[k]);
     }
   }
-  printf("optim_emu_test: %d checks, %d failures, worst error/bound %.3f\n", g_checks, g_fail, g_worst);
+}
+
+// ------------------------------------------------------------------ SGD
+// One element through several steps: the kernel body (sgd_update, fed g, or fl(scratch * coef) on the clipped path)
+// and a long-double torch.optim.SGD fed the same fp32 inputs and hyper-parameters, with G = g * coef * gscale:
+//   d = wd p + G,   b' = mu b + d,   p' = p - lr b'
+// with torch's treatment of zero hyper-parameters: d = G when wd = 0 (p is not read), b' = d when mu = 0 (no buffer).
+// The kernel rounds g*gscale, the fmaf for d, the fmaf for b' and the one for p' (and scratch*coef before them on the
+// clipped path).  To first order, with the bounds B of the step before carried forward:
+//   B_d  = wd B_p + u(wd|p| + k|G|) + F             (k = 2, or 3 on the clipped path)
+//   B_b' = mu B_b + B_d + u(mu|b| + |d|) + F
+//   B_p' = B_p + lr B_b' + u(|p| + lr|b'|) + F
+struct SgdHp { float lr, mu, wd, gs; };
+
+struct SgdElem {
+  float p, b;          // kernel state
+  LD rp, rb;           // reference state
+  LD Bp, Bb;           // bounds of |p - rp|, |b - rb|
+};
+
+static SgdElem sgd_elem(float p, float b) { return SgdElem{p, b, (LD)p, (LD)b, 0, 0}; }
+
+static double s_worst = 0.0;
+
+static void sgd_check(const char* what, float got, LD want, LD bound, const char* label, const SgdHp& h, float g) {
+  if (isnan(want) || isinf(want)) {
+    const bool ok = isnan(want) ? isnan(got) : (LD)got == want;
+    CHECK(ok, "sgd %s: %s got %g want %Lg (g=%g lr=%g mu=%g wd=%g gs=%g)", label, what, got, want, g, h.lr, h.mu, h.wd, h.gs);
+    return;
+  }
+  const LD err = fabsl((LD)got - want);
+  // after a non-finite step the carried bound is no longer finite; a finite reference value then needs a finite result
+  const bool ok = isfinite(got) && (!isfinite(bound) || err <= bound);
+  CHECK(ok, "sgd %s: %s got %.9g want %.12Lg err %Lg bound %Lg (g=%g lr=%g mu=%g wd=%g gs=%g)", label, what, got, want, err,
+        bound, g, h.lr, h.mu, h.wd, h.gs);
+  if (ok && isfinite(bound) && bound > 0) s_worst = fmax(s_worst, (double)(err / bound));
+}
+
+// one step of element `e`; coef < 0: the one-kernel path, else the clipped path with that coefficient
+static void sgd_step(SgdElem& e, const SgdHp& h, float g, float coef, const char* label) {
+  const bool clipped = coef >= 0.0f;
+  sgd_update(clipped ? g * coef : g, e.p, e.b, h.lr, h.mu, h.wd, h.gs);
+
+  const LD lr = h.lr, mu = h.mu, wd = h.wd;
+  const LD G = (LD)g * (clipped ? (LD)coef : 1.0L) * (LD)h.gs;
+  const LD d = h.wd == 0.0f ? G : wd * e.rp + G;
+  const LD b1 = h.mu == 0.0f ? d : mu * e.rb + d;
+  const LD p1 = e.rp - lr * b1;
+  const LD Bd = wd * e.Bp + kU * (wd * fabsl(e.rp) + (clipped ? 3 : 2) * fabsl(G)) + kF;
+  const LD Bb = mu * e.Bb + Bd + kU * (mu * fabsl(e.rb) + fabsl(d)) + kF;
+  const LD Bp = e.Bp + lr * Bb + kU * (fabsl(e.rp) + lr * fabsl(b1)) + kF;
+  e.rp = p1, e.rb = b1, e.Bp = Bp, e.Bb = Bb;
+  sgd_check("p", e.p, e.rp, e.Bp, label, h, g);
+  sgd_check("buf", e.b, e.rb, e.Bb, label, h, g);
+}
+
+static void sgd_checks() {
+  const SgdHp bases[] = {
+      {0.1f, 0.9f, 1e-2f, 1.f},          // momentum and weight decay
+      {0.05f, 0.f, 0.f, 0.5f},           // plain SGD (no buffer in torch), gradient averaged over 2 ranks
+      {0.1f, 0.9f, 0.f, 1.f / 3},        // a gradient scale that is not a power of two (3 ranks)
+      {0.f, 0.9f, 1e-2f, 1.f},           // lr = 0: the parameters stay, the buffer still moves
+  };
+  const float coefs[] = {-1.f, 0.3f, 1e-3f, 1.f, 0.f};     // the one-kernel path, then clipped with these coefficients
+  // gradient classes: ordinary, tiny (subnormal products), huge, zero
+  const struct { const char* name; float scale; } classes[] = {{"ordinary", 3.f}, {"tiny", 1e-36f}, {"huge", 1e30f}, {"zero", 0.f}};
+  const float lr_sched[] = {1.f, 1.f, 0.3f, 0.3f, 0.1f};   // the learning rate changes between steps
+  for (const SgdHp& h0 : bases)
+    for (const float coef : coefs)
+      for (const auto& cl : classes)
+        for (int i = 0; i < 400; i++) {
+          // state of the gradients' magnitude (half the time), or left over from larger ones; 5 steps
+          const float ss = (i & 1) ? cl.scale : 1.f;
+          SgdElem e = sgd_elem(srand_(2.f), (i & 2) ? srand_(ss) : 0.f);
+          for (const float f : lr_sched) {
+            SgdHp h = h0;
+            h.lr = h0.lr * f;
+            sgd_step(e, h, srand_(cl.scale), coef, cl.name);
+          }
+        }
+  // NaN and +-Inf in g and in the buffer, one step from finite p
+  const float specials[] = {NAN, INFINITY, -INFINITY};
+  for (const SgdHp& h : bases)
+    for (const float coef : coefs)
+      for (const float s : specials) {
+        SgdElem a = sgd_elem(0.5f, 0.01f), b = sgd_elem(0.5f, s), c = sgd_elem(0.5f, s);
+        sgd_step(a, h, s, coef, "g special");
+        sgd_step(b, h, 0.3f, coef, "buf special");
+        sgd_step(c, h, s, coef, "all special");
+      }
+  // momentum 0 after an infinite gradient: torch steps with d_p alone, so the element stays at its infinity (or NaN)
+  // and the next finite gradients do not turn it into NaN
+  const float decays[] = {0.f, 1e-2f};
+  for (const float wd : decays)
+    for (const float s : specials) {
+      const SgdHp h = {0.1f, 0.f, wd, 1.f};
+      SgdElem e = sgd_elem(0.5f, 0.f), f = sgd_elem(0.5f, 0.f);
+      sgd_step(e, h, s, -1.f, "mu=0 sequence");
+      sgd_step(f, h, 0.3f, -1.f, "mu=0 sequence");
+      for (int k = 0; k < 2; k++) {
+        sgd_step(e, h, 0.3f, -1.f, "mu=0 sequence");
+        sgd_step(f, h, 0.3f, -1.f, "mu=0 sequence");
+      }
+      if (wd == 0.f) {
+        CHECK(isnan(s) ? isnan(e.p) : e.p == -s, "mu=0: p=%g after g=%g", e.p, s);
+        CHECK(isfinite(e.b) && e.b == 0.3f, "mu=0: buf=%g (d_p of the last step)", e.b);
+      }
+      CHECK(isfinite(f.p), "mu=0: neighbour p=%g", f.p);
+    }
+}
+
+int main() {
+  adamw_checks();
+  const int adamw = g_checks;
+  printf("optim_emu_test: adamw %d checks, worst error/bound %.3f\n", adamw, g_worst);
+  sgd_checks();
+  printf("optim_emu_test: sgd %d checks, worst error/bound %.3f\n", g_checks - adamw, s_worst);
+  printf("optim_emu_test: %d checks, %d failures\n", g_checks, g_fail);
   if (g_fail) return 1;
   printf("optim_emu_test: ok\n");
   return 0;

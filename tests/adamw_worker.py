@@ -1,6 +1,7 @@
 """Per-rank bodies of the fused AdamW GPU tests (launched by tests/test_fused_adamw.py, one process per GPU)."""
 from __future__ import annotations
 
+import math
 import os
 import sys
 
@@ -92,7 +93,9 @@ class Reference:
         """Largest error/bound ratio of the three fp32 tensors."""
         r = 0.0
         for got, want, b in ((master, self.p, self.bp), (exp_avg, self.m, self.bm), (exp_avg_sq, self.v, self.bv)):
-            r = max(r, float(((got.double() - want).abs() / b).max()))
+            # (a NaN or infinite result where the reference is finite counts as outside the bound: torch's max() of a
+            # tensor with a NaN is NaN, and Python's max(r, nan) would drop it)
+            r = max(r, float(((got.double() - want).abs() / b).nan_to_num(nan=math.inf, posinf=math.inf).max()))
         return r
 
 

@@ -62,10 +62,6 @@ def test_executor_relaunch_after_idle():
 
 
 # ------------------------------------------------------------------ fused optimizer / DDP engine, single GPU
-def test_fused_sgd_matches_torch_single_gpu():
-    _run_worker("fused_sgd", 1)
-
-
 def test_ddp_engine_trains_like_torch_sgd():
     _run_worker("ddp_engine", 1)
 
@@ -102,11 +98,6 @@ def test_bench_contract_single_gpu():
 @pytest.mark.multigpu
 def test_allreduce_kernels_2gpu():
     _run_worker("allreduce", 2)
-
-
-@pytest.mark.multigpu
-def test_fused_sgd_2gpu_matches_reference():
-    _run_worker("fused_sgd", 2)
 
 
 @pytest.mark.multigpu
