@@ -80,6 +80,7 @@ def _declare(lib):
     lib.bnet_fused_allreduce_sgd_hp.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, i, i, i, vp]
     lib.bnet_fused_allreduce_adamw.argtypes = [vp, sz, sz, sz, i, vp, vp, vp, vp, i, i, i, vp]
     lib.bnet_fused_clip_reduce_norm.argtypes = [vp, sz, sz, i, vp, vp, i, i, vp]
+    lib.bnet_fused_accum_reduce_norm.argtypes = [vp, sz, sz, i, vp, vp, i, i, vp]
     lib.bnet_fused_clip_coef.argtypes = [vp, vp, i, sz, C.c_float, vp, i, vp]
     lib.bnet_fused_clip_apply_sgd.argtypes = [vp, sz, sz, i, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp, i, i, vp]
     lib.bnet_fused_clip_apply_sgd_hp.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, vp, i, i, vp]
@@ -285,6 +286,18 @@ class SymmComm:
         n = self._chk(self.lib.bnet_fused_clip_reduce_norm(
             self.h, self.offset_of(grad), grad.numel(), DT[grad.dtype], C.c_void_p(scratch.data_ptr()),
             C.c_void_p(partial.data_ptr()), channel, nblocks, self._stream(stream)), "fused_clip_reduce_norm")
+        self.launches += n
+
+    def fused_accum_reduce_norm(self, grad: torch.Tensor, scratch: torch.Tensor, partial: torch.Tensor, channel: int = 0,
+                                nblocks: int = 0, stream=None):
+        """Stage 1 of a micro-batch that accumulates (gradient accumulation): like ``fused_clip_reduce_norm``, but ADD the
+        rank-summed ``grad`` to this rank's fp32 ``scratch`` shard (scratch + g, in fp32); ``partial`` gets the sums of
+        squares of the new scratch values.  Zeroes ``grad``."""
+        assert scratch.dtype == torch.float32 and scratch.is_contiguous() and scratch.numel() * self.world == grad.numel()
+        assert partial.is_cuda and partial.dtype == torch.float64 and partial.is_contiguous() and partial.numel() >= CLIP_ROW
+        n = self._chk(self.lib.bnet_fused_accum_reduce_norm(
+            self.h, self.offset_of(grad), grad.numel(), DT[grad.dtype], C.c_void_p(scratch.data_ptr()),
+            C.c_void_p(partial.data_ptr()), channel, nblocks, self._stream(stream)), "fused_accum_reduce_norm")
         self.launches += n
 
     def fused_clip_coef(self, partials: torch.Tensor, xchg: torch.Tensor, clip: torch.Tensor, grad_scale: float | None = None,

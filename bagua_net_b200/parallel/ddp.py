@@ -151,9 +151,9 @@ class _Bucket:
         self.start = 0
         self.numel = 0
         self.ready = 0
-        self.scratch = None          # clipped step: this rank's fp32 shard of the rank-summed gradient
-        self.partial = None          # clipped step: the bucket's row of per-CTA sums of squares
-        self.launched = False        # clipped step: stage 1 ran for this bucket in the current step
+        self.scratch = None          # staged step: this rank's fp32 shard of the rank-summed (accumulated) gradient
+        self.partial = None          # staged step: the bucket's row of per-CTA sums of squares
+        self.launched = False        # staged step: stage 1 ran for this bucket in the current step (the scratch holds data)
 
     @property
     def master(self) -> torch.Tensor:
@@ -171,13 +171,25 @@ class BnetDDP(torch.nn.Module):
     ``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)`` does (``inf`` computes the norm and never clips).  The step
     then runs in three stages: per bucket from the gradient hook, reduce into an fp32 scratch and sum squares; once per
     step, the norm and the coefficient; per bucket, the update from the scratch.  ``None`` keeps the one-kernel step.
+
+    accumulation_steps: gradient accumulation over k micro-batches per optimizer step.  ``train_step`` splits its batch
+    along dim 0 into k equal micro-batches, runs k forward/backward passes and one update, and returns the mean of the k
+    losses.  Every micro-batch's gradients are reduced over the ranks while its backward runs and summed in this rank's
+    fp32 scratch shard; the update (and clipping) runs once, on the k-th ``finish_step``, with the gradient scaled by
+    1/(world * k): the gradient of the mean loss over the global batch.  In a loop of your own, call
+    ``loss.backward(); engine.finish_step()`` once per micro-batch with the UNSCALED micro-batch loss (the mean over the
+    micro-batch) -- do not divide it by k, the engine does that.  ``micro_step`` tells where in the step you are.
+    BatchNorm statistics are per micro-batch, as with accumulation in torch.  ``1`` keeps the single-batch step.
     """
 
     def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float | None = None, weight_decay: float = 0.0,
                  bucket_mb: float = 64.0, comm: SymmComm | None = None, extra_heap_bytes: int = 64 << 20,
                  nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
-                 eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None):
+                 eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None,
+                 accumulation_steps: int = 1):
         super().__init__()
+        if isinstance(accumulation_steps, bool) or not isinstance(accumulation_steps, int) or accumulation_steps < 1:
+            raise ValueError(f"accumulation_steps must be an int >= 1 (got {accumulation_steps!r})")
         if max_grad_norm is not None:
             max_grad_norm = _check_max_norm(max_grad_norm)
         if optimizer not in ("sgd", "adamw"):
@@ -232,6 +244,10 @@ class BnetDDP(torch.nn.Module):
         if comm is None:
             comm = SymmComm(2 * total * es + extra_heap_bytes + (1 << 20), device=dev.index, group=group)
         self.comm = comm
+        self.accumulation_steps = accumulation_steps
+        self._micro = 0
+        # the mean gradient over the global batch: world ranks times k micro-batches (for k = 1 exactly 1/world, as before)
+        self._grad_scale = 1.0 / (comm.world * accumulation_steps)
         self.flat_param = comm.alloc(total, dtype)
         self.flat_grad = comm.alloc(total, dtype)
         self.flat_param.zero_()
@@ -289,17 +305,23 @@ class BnetDDP(torch.nn.Module):
         # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh); SGD
         # passes them as launch arguments until the first set_lr
         self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev) if optimizer == "adamw" else None
-        # gradient clipping: per bucket an fp32 scratch shard and a row of per-CTA partial sums of squares, one exchange
-        # area in the heap (same offset on every rank) and the device block {max_norm, total_norm, clip_coef, reserved}
+        # the staged step (gradient clipping, gradient accumulation, or both): per bucket an fp32 scratch shard and a row
+        # of per-CTA partial sums of squares.  Clipping adds one exchange area in the heap (same offset on every rank) and
+        # the device block {max_norm, total_norm, clip_coef, reserved}; accumulation without clipping updates through the
+        # constant block {inf, 0, 1, 0} instead (clip_coef exactly 1).
         self._clip = None
-        if max_grad_norm is not None:
+        self._staged = max_grad_norm is not None or accumulation_steps > 1
+        if self._staged:
             from .comm import CLIP_ROW
 
             self._partials = torch.zeros(len(self.buckets), CLIP_ROW, dtype=torch.float64, device=dev)
             for b, row in zip(self.buckets, self._partials):
                 b.scratch, b.partial = torch.zeros_like(b.master), row
+        if max_grad_norm is not None:
             self._xchg = comm.alloc(comm.world, torch.float64)
             self._clip = torch.tensor([max_grad_norm, 0.0, 0.0, 0.0], dtype=torch.float32, device=dev)
+        elif accumulation_steps > 1:
+            self._coef_one = torch.tensor([float("inf"), 0.0, 1.0, 0.0], dtype=torch.float32, device=dev)
         self.max_grad_norm = max_grad_norm
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
@@ -329,9 +351,10 @@ class BnetDDP(torch.nn.Module):
         ev = torch.cuda.Event()
         ev.record(cur)
         self.comm_stream.wait_event(ev)          # the bucket's gradients are complete on the compute stream
-        if self._clip is not None:               # clipped step, stage 1: reduce into the scratch, sum of squares
-            self.comm.fused_clip_reduce_norm(b.grad, b.scratch, b.partial, channel=0, nblocks=self.nblocks,
-                                             stream=self.comm_stream)
+        if self._staged:                         # staged step, stage 1: reduce into the scratch, sum of squares
+            # the bucket's first contribution in this step stores, every later micro-batch's adds to it
+            stage1 = self.comm.fused_accum_reduce_norm if b.launched else self.comm.fused_clip_reduce_norm
+            stage1(b.grad, b.scratch, b.partial, channel=0, nblocks=self.nblocks, stream=self.comm_stream)
             b.launched = True
         elif self.optimizer == "adamw":
             self.comm.fused_allreduce_adamw(b.grad, b.param, *b.state, self._hp, zero_grads=True, channel=0,
@@ -344,13 +367,23 @@ class BnetDDP(torch.nn.Module):
         self._inflight = True
 
     def finish_step(self):
-        """Make the updated parameters visible to the compute stream (call after backward)."""
+        """Make the updated parameters visible to the compute stream (call after backward).  With
+        ``accumulation_steps=k``, call it after every micro-batch's backward: the first k-1 calls only reduce that
+        micro-batch's gradients into the scratch, the k-th also updates."""
         for b in self.buckets:
             if b.ready:                           # parameters that got no gradient this step
                 self._launch(b)
+        if self.accumulation_steps > 1:
+            self._micro += 1
+            if self._micro < self.accumulation_steps:
+                # the next backward writes into gradient slices that this micro-batch's stage 1 zeroes
+                if self._inflight:
+                    torch.cuda.current_stream().wait_stream(self.comm_stream)
+                return
+            self._micro = 0
         if self._inflight:
-            if self._clip is not None:
-                self._clipped_update()
+            if self._staged:
+                self._staged_update()
             if self.optimizer == "adamw":
                 # one optimizer step taken: advance the step count the kernels read, behind this step's last bucket
                 # (on the comm stream, so a captured step replays it)
@@ -359,8 +392,9 @@ class BnetDDP(torch.nn.Module):
             torch.cuda.current_stream().wait_stream(self.comm_stream)
             self._inflight = False
 
-    def _clipped_update(self):
-        """Stages 2 and 3 of the clipped step, on the comm stream behind every bucket's stage 1."""
+    def _staged_update(self):
+        """Stages 2 and 3 of the staged step (clipping and/or accumulation), on the comm stream behind every bucket's
+        stage 1, once per optimizer step."""
         # Behind the whole backward: stage 2's rank barrier then also means that every rank's backward is done, which
         # is what lets stage 3 write new parameters into the peers without an opening barrier of its own.
         self.comm_stream.wait_stream(torch.cuda.current_stream())
@@ -368,17 +402,26 @@ class BnetDDP(torch.nn.Module):
             for b in self.buckets:
                 if not b.launched:                # no gradient at all this step: no update, and nothing in the norm
                     b.partial.zero_()
-        self.comm.fused_clip_coef(self._partials, self._xchg, self._clip, channel=0, stream=self.comm_stream)
+        if self._clip is not None:
+            self.comm.fused_clip_coef(self._partials, self._xchg, self._clip, grad_scale=self._grad_scale, channel=0,
+                                      stream=self.comm_stream)
+            coef = self._clip
+        else:
+            # accumulation without clipping: only the barrier, and a coefficient of exactly 1.  (Not the coefficient
+            # kernel at max_norm = inf: that turns a NaN norm into a NaN coefficient for every element, where an
+            # unclipped torch step poisons only the NaN elements.)
+            self.comm.barrier(channel=0, stream=self.comm_stream)
+            coef = self._coef_one
         for b in self.buckets:
             if not b.launched:
                 continue
             if self.optimizer == "adamw":
-                self.comm.fused_clip_apply_adamw(b.param, b.scratch, self._clip, *b.state, self._hp, channel=0,
+                self.comm.fused_clip_apply_adamw(b.param, b.scratch, coef, *b.state, self._hp, channel=0,
                                                  nblocks=self.nblocks, stream=self.comm_stream)
             else:
-                self.comm.fused_clip_apply_sgd(b.param, b.scratch, self._clip, *b.state, self.lr, self.momentum,
-                                               self.weight_decay, channel=0, nblocks=self.nblocks, stream=self.comm_stream,
-                                               hp=self._hp)
+                self.comm.fused_clip_apply_sgd(b.param, b.scratch, coef, *b.state, self.lr, self.momentum,
+                                               self.weight_decay, self._grad_scale, channel=0, nblocks=self.nblocks,
+                                               stream=self.comm_stream, hp=self._hp)
             b.launched = False
 
     # ------------------------------------------------------------------ user API
@@ -386,11 +429,21 @@ class BnetDDP(torch.nn.Module):
         return self.module(*args, **kwargs)
 
     def _eager_step(self, inputs, targets, loss_fn):
-        out = self.module(inputs)
-        loss = loss_fn(out.float(), targets)
-        loss.backward()
-        self.finish_step()
-        return loss.detach()
+        k = self.accumulation_steps
+        if k == 1:
+            out = self.module(inputs)
+            loss = loss_fn(out.float(), targets)
+            loss.backward()
+            self.finish_step()
+            return loss.detach()
+        # k micro-batches: equal views along dim 0 (the slices of a channels_last batch are channels_last)
+        losses = []
+        for x, y in zip(inputs.split(inputs.shape[0] // k), targets.split(targets.shape[0] // k)):
+            loss = loss_fn(self.module(x).float(), y)
+            loss.backward()
+            self.finish_step()
+            losses.append(loss.detach())
+        return torch.stack(losses).mean()
 
     def enable_cuda_graph(self, enabled: bool = True):
         """Capture forward + backward + the fused collective/optimizer kernels (both streams) into ONE
@@ -420,6 +473,7 @@ class BnetDDP(torch.nn.Module):
             saved = [t.clone() for t in live]
             for _ in range(2):
                 self._eager_step(self._gx, self._gy, loss_fn)
+            self._micro = 0                         # (two whole steps: back at the first micro-batch already)
             torch.cuda.current_stream().synchronize()
             if self.comm.world > 1:
                 dist.barrier()                      # nobody restores while a peer's kernel still writes parameters
@@ -443,7 +497,16 @@ class BnetDDP(torch.nn.Module):
             dist.barrier()
 
     def train_step(self, inputs: torch.Tensor, targets: torch.Tensor, loss_fn=None) -> torch.Tensor:
-        """forward + backward + fused all-reduce/optimizer.  Returns the (device) loss tensor."""
+        """forward + backward + fused all-reduce/optimizer.  Returns the (device) loss tensor.  With
+        ``accumulation_steps=k``: k micro-batches of ``inputs.shape[0] // k`` samples and one update; the loss returned
+        is the mean of the k micro-batch losses."""
+        k = self.accumulation_steps
+        if self._micro:
+            raise ValueError(f"train_step called in the middle of an accumulation step (micro_step={self._micro}): "
+                             "finish that step with backward + finish_step first")
+        if k > 1 and (inputs.shape[0] % k or targets.shape[0] != inputs.shape[0]):
+            raise ValueError(f"a batch of {inputs.shape[0]} inputs / {targets.shape[0]} targets does not split into "
+                             f"accumulation_steps={k} equal micro-batches")
         loss_fn = loss_fn or torch.nn.functional.cross_entropy
         if not getattr(self, "_use_graph", False):
             return self._eager_step(inputs, targets, loss_fn)
@@ -543,7 +606,13 @@ class BnetDDP(torch.nn.Module):
     # Model weights live in ordinary nn.Module tensors (views into the flat heap), so module.state_dict() /
     # load_state_dict() work unchanged.  The optimizer state is this rank's 1/world shard of the fp32 master
     # weights and momentum (SGD) or exp_avg / exp_avg_sq (AdamW, which also saves its step count) of every bucket.
+    def _check_step_boundary(self, what: str) -> None:
+        if self._micro:
+            raise ValueError(f"cannot {what} in the middle of an accumulation step (micro_step={self._micro}): the "
+                             "scratch holds a partial gradient sum that is not saved")
+
     def optimizer_state_dict(self) -> dict:
+        self._check_step_boundary("save the optimizer state")
         if self.optimizer == "adamw":
             head = {"optimizer": "adamw", "lr": self.lr, "betas": self.betas, "eps": self.eps,
                     "weight_decay": self.weight_decay, "step": int(self._hp[self._HP_STEP].item())}
@@ -554,6 +623,7 @@ class BnetDDP(torch.nn.Module):
                 "buckets": [{k: t.detach().cpu() for k, t in zip(names, b.state)} for b in self.buckets]}
 
     def load_optimizer_state_dict(self, state: dict) -> None:
+        self._check_step_boundary("load an optimizer state")
         kind = state.get("optimizer", "sgd")
         if kind != self.optimizer:
             raise ValueError(f"optimizer state of {kind!r} cannot be loaded into a {self.optimizer!r} engine")
@@ -610,7 +680,7 @@ class BnetDDP(torch.nn.Module):
             self.momentum = float(momentum)
         if weight_decay is not None:
             self.weight_decay = float(weight_decay)
-        vals = [self.lr, self.momentum, self.weight_decay, 1.0 / self.comm.world]
+        vals = [self.lr, self.momentum, self.weight_decay, self._grad_scale]
         if self._hp is None:
             self._hp = torch.tensor(vals, dtype=torch.float32, device=self.flat_param.device)
             self._graph = None
@@ -636,11 +706,16 @@ class BnetDDP(torch.nn.Module):
     _HP_STEP = 6
 
     def _adamw_hp(self, step: int) -> list:
-        return [self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, 1.0 / self.comm.world, float(step), 0.0]
+        return [self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, self._grad_scale, float(step), 0.0]
 
     def _state(self, b: _Bucket) -> tuple:
         """The fp32 tensors the fused kernel updates for bucket `b`, master first."""
         return b.state
+
+    @property
+    def micro_step(self) -> int:
+        """The micro-batch of the current optimizer step that the next backward belongs to (0..accumulation_steps-1)."""
+        return self._micro
 
     @property
     def kernel_launches(self) -> int:

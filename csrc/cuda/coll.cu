@@ -639,9 +639,15 @@ __device__ __forceinline__ double cta_sum(double v) {
 // to its own slot of the bucket's `partial` row (BNET_COLL_MAX_BLOCKS doubles; CTA 0 zeroes the slots beyond the
 // grid).  No atomics: the same grid gives the same bits.  Squares and sums are taken in double: a square of an fp32
 // value is exact there, and a sum of n of them is within n * 2^-53 of the exact one.
-template <int DT, int MODE>
-__global__ void __launch_bounds__(kThreads, 2) bnet_clip_norm_kernel(CollDev d, size_t goff, size_t nvec, float* __restrict__ scratch,
-                                                                 double* __restrict__ partial, int chan) {
+//
+// ACC (gradient accumulation, every micro-batch after a bucket's first in the step): add the rank-summed gradient to
+// what `scratch` already holds (scratch + g, in fp32) instead of storing it, and take the sums of squares over the new
+// scratch values, so the bucket's partial row always describes its accumulated gradient.  The scratch loads are issued
+// together with the gradient loads, before any dependent math, as fused_batch does; they go first because with peer
+// loads (MODE 2) fused_grad_issue already sums, and in this order the bf16 P2P variant fits 64 registers unspilled.
+template <int DT, int MODE, bool ACC>
+__device__ __forceinline__ void reduce_norm_body(const CollDev& d, size_t goff, size_t nvec, float* __restrict__ scratch,
+                                                 double* __restrict__ partial, int chan) {
   constexpr int E = VecTraits<DT>::kElems;
   constexpr int Q = E / 4;
   constexpr int U = 2;
@@ -653,14 +659,28 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_clip_norm_kernel(CollDev d, 
   for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < per; i += U * stride) {
     int4 gv[U];
     float gp2p[(MODE == 2) ? U : 1][8];
+    float4 sv[ACC ? U : 1][Q];
 #pragma unroll
-    for (int u = 0; u < U; u++)
-      if (i + u * stride < per) fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
+    for (int u = 0; u < U; u++) {
+      if (i + u * stride >= per) continue;
+      if constexpr (ACC) {
+#pragma unroll
+        for (int q = 0; q < Q; q++) sv[u][q] = ptx::ld_na_f4(reinterpret_cast<const float4*>(scratch + (i + u * stride) * E) + q);
+      }
+      fused_grad_issue<DT, MODE>(d, goff + (start + i + u * stride) * 16, gv[u], gp2p[(MODE == 2) ? u : 0]);
+    }
 #pragma unroll
     for (int u = 0; u < U; u++) {
       if (i + u * stride >= per) continue;
       float g[8];
       fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
+      if constexpr (ACC) {
+#pragma unroll
+        for (int q = 0; q < Q; q++) {
+          g[4 * q] = sv[u][q].x + g[4 * q]; g[4 * q + 1] = sv[u][q].y + g[4 * q + 1];
+          g[4 * q + 2] = sv[u][q].z + g[4 * q + 2]; g[4 * q + 3] = sv[u][q].w + g[4 * q + 3];
+        }
+      }
 #pragma unroll
       for (int q = 0; q < Q; q++)
         ptx::st_na_f4(reinterpret_cast<float4*>(scratch + (i + u * stride) * E) + q,
@@ -675,6 +695,19 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_clip_norm_kernel(CollDev d, 
     for (int j = gridDim.x + threadIdx.x; j < BNET_COLL_MAX_BLOCKS; j += kThreads) partial[j] = 0.0;
   if constexpr (MODE != 0) rank_barrier(d, chan);
   fused_zero_grads(d, goff, nvec, per, stride);
+}
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_norm_kernel(CollDev d, size_t goff, size_t nvec, float* __restrict__ scratch,
+                                                                 double* __restrict__ partial, int chan) {
+  reduce_norm_body<DT, MODE, false>(d, goff, nvec, scratch, partial, chan);
+}
+
+// Stage 1 of an accumulating micro-batch: scratch += the rank-summed gradient (reduce_norm_body with ACC).
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_accum_norm_kernel(CollDev d, size_t goff, size_t nvec, float* __restrict__ scratch,
+                                                                  double* __restrict__ partial, int chan) {
+  reduce_norm_body<DT, MODE, true>(d, goff, nvec, scratch, partial, chan);
 }
 
 // Stage 2, one CTA per step after the last bucket's stage 1: sum this rank's `n` partials (all its rows) in a fixed
@@ -1336,6 +1369,9 @@ BNET_API int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t par
 struct ClipNormKernel {
   template <int DT, int MODE> static constexpr auto fn = bnet_clip_norm_kernel<DT, MODE>;
 };
+struct AccumNormKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_accum_norm_kernel<DT, MODE>;
+};
 struct ClipSgdKernel {
   template <int DT, int MODE> static constexpr auto fn = bnet_clip_apply_sgd_kernel<DT, MODE>;
 };
@@ -1354,6 +1390,14 @@ BNET_API int bnet_fused_clip_reduce_norm(BnetColl* c, size_t grad_off, size_t co
   FusedLaunch f;
   if (fused_prologue(c, "clip norm", grad_off, grad_off, count, dtype, channel, {scratch}, nblocks, stream, f) < 0) return -1;
   return run_fused_kernel<ClipNormKernel>(c, dtype, f, f.goff, f.nvec, scratch, partial, channel);
+}
+
+BNET_API int bnet_fused_accum_reduce_norm(BnetColl* c, size_t grad_off, size_t count, int dtype, float* scratch, double* partial,
+                                          int channel, int nblocks, void* stream) {
+  if (!partial || ((uintptr_t)partial & 7)) return fail("partial row must be an 8-byte aligned device pointer");
+  FusedLaunch f;
+  if (fused_prologue(c, "accumulating norm", grad_off, grad_off, count, dtype, channel, {scratch}, nblocks, stream, f) < 0) return -1;
+  return run_fused_kernel<AccumNormKernel>(c, dtype, f, f.goff, f.nvec, scratch, partial, channel);
 }
 
 BNET_API int bnet_fused_clip_coef(BnetColl* c, const double* partials, int nrows, size_t xchg_off, float grad_scale, float* clip,

@@ -20,14 +20,16 @@ def batches(n, batch, device_rank):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--batch", type=int, default=32, help="images per rank and optimizer step")
+    ap.add_argument("--accumulation-steps", type=int, default=1,
+                    help="split every batch into this many micro-batches (one forward/backward each) and update once")
     ap.add_argument("--model", default="vgg16")
     ap.add_argument("--checkpoint", default="")
     a = ap.parse_args()
     init_process_group_from_env()
     rank = int(os.environ.get("RANK", "0"))
     model = build_model(a.model, fused=True).cuda().bfloat16().to(memory_format=torch.channels_last)
-    engine = BnetDDP(model, lr=0.01, momentum=0.9, weight_decay=1e-4)
+    engine = BnetDDP(model, lr=0.01, momentum=0.9, weight_decay=1e-4, accumulation_steps=a.accumulation_steps)
     engine.enable_cuda_graph(True)            # forward + backward + every bucket kernel replay as one graph
     engine.set_lr(0.01)                       # hyper-parameters live in device memory: the graph follows the schedule
     for step, loss in enumerate(engine.train_from_host(batches(a.steps, a.batch, rank))):

@@ -108,6 +108,11 @@ int bnet_fused_allreduce_adamw(BnetColl* c, size_t grad_off, size_t param_off, s
 #define BNET_COLL_CLIP_ROW BNET_COLL_MAX_BLOCKS
 int bnet_fused_clip_reduce_norm(BnetColl* c, size_t grad_off, size_t count, int dtype, float* scratch, double* partial,
                                 int channel, int nblocks, void* stream);
+/* Stage 1 of a micro-batch that accumulates (gradient accumulation, every micro-batch after the bucket's first in the
+ * step): the same reduction and checks, but scratch[i] = scratch[i] + sum (fp32), the partial row gets the sums of
+ * squares of the NEW scratch values, and grad[bucket] is zeroed.  Same determinism. */
+int bnet_fused_accum_reduce_norm(BnetColl* c, size_t grad_off, size_t count, int dtype, float* scratch, double* partial,
+                                 int channel, int nblocks, void* stream);
 /* Stage 2, once per step after every bucket's stage 1 (and after the caller's stream has waited for backward): sum the
  * nrows x BNET_COLL_CLIP_ROW doubles at `partials` in a fixed order, exchange the per-rank sums through `world` doubles at
  * heap byte offset `xchg_off` (16-byte aligned, same offset on every rank, used by nothing else) and add them in rank
