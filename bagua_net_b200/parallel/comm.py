@@ -26,6 +26,42 @@ OPS = {"sum": 0, "avg": 1, "max": 2, "min": 3}
 ALGOS = {"auto": 0, "nvls": 1, "p2p": 2, "oneshot": 3, "ll": 0}
 BLOB = 128
 CLIP_ROW = 304          # doubles per bucket in the clipped step's partial rows (BNET_COLL_CLIP_ROW)
+LARS_CHUNK = 4096       # vectors per norm slot of the LARS norm pass (BNET_LARS_CHUNK)
+
+
+def check_lars_segments(table, shard_vecs: int, ntensors: int) -> int:
+    """Validate a LARS segment table (rows {vec0, nvec, tensor, slot0}, see include/bnet/bnet_coll.h) for a shard of
+    `shard_vecs` 16-byte vectors before it goes to the device, where the kernels trust it: sorted, in range, covering the
+    shard exactly once, tensor indices below `ntensors`, slot0 the running count of BNET_LARS_CHUNK chunks.  Returns the
+    number of norm slots; raises ValueError."""
+    rows = [tuple(int(v) for v in r) for r in torch.as_tensor(table).reshape(-1, 4).tolist()]
+    if not rows:
+        raise ValueError("LARS segment table is empty")
+    if not 0 < shard_vecs < 2 ** 31:
+        raise ValueError(f"LARS shard of {shard_vecs} vectors is out of range")
+    pos, slots = 0, 0
+    for k, (vec0, nvec, tensor, slot0) in enumerate(rows):
+        if vec0 != pos or nvec < 1 or pos + nvec > shard_vecs:
+            raise ValueError(f"LARS segment {k} ({vec0}, {nvec}) does not continue the cover of the shard at vector {pos}")
+        if not 0 <= tensor < ntensors:
+            raise ValueError(f"LARS segment {k} names tensor {tensor} of {ntensors}")
+        if slot0 != slots:
+            raise ValueError(f"LARS segment {k} starts at slot {slot0}, expected {slots}")
+        pos += nvec
+        slots += (nvec + LARS_CHUNK - 1) // LARS_CHUNK
+    if pos != shard_vecs:
+        raise ValueError(f"LARS segments cover {pos} of the shard's {shard_vecs} vectors")
+    return slots
+
+
+def check_lars_tensors(table, nslots: int) -> None:
+    """Validate a LARS tensor table (rows {slot0, nslots, excluded, reserved}): every slot range inside `nslots`."""
+    rows = torch.as_tensor(table).reshape(-1, 4).tolist()
+    if not rows:
+        raise ValueError("LARS tensor table is empty")
+    for j, (slot0, n, _, _) in enumerate(rows):
+        if n < 0 or slot0 < 0 or slot0 + n > nslots:
+            raise ValueError(f"LARS tensor {j}: slots [{slot0}, {slot0 + n}) outside the {nslots} slots")
 
 
 def _host_identity():
@@ -85,6 +121,9 @@ def _declare(lib):
     lib.bnet_fused_clip_apply_sgd.argtypes = [vp, sz, sz, i, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp, i, i, vp]
     lib.bnet_fused_clip_apply_sgd_hp.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, vp, i, i, vp]
     lib.bnet_fused_clip_apply_adamw.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, vp, vp, i, i, vp]
+    lib.bnet_fused_lars_norm.argtypes = [vp, sz, i, vp, vp, vp, i, vp, i, i, vp]
+    lib.bnet_fused_lars_trust.argtypes = [vp, vp, vp, i, sz, vp, vp, vp, vp, i, vp]
+    lib.bnet_fused_lars_apply.argtypes = [vp, sz, sz, i, vp, vp, i, vp, vp, vp, vp, i, i, vp]
     lib.bnet_pack_cast.argtypes = [vp, i, vp, i, i, C.c_float, C.c_uint64, vp]
 
 
@@ -135,6 +174,7 @@ class SymmComm:
         self.has_multicast = bool(self.lib.bnet_coll_has_multicast(self.h))
         self._heap = torch.as_tensor(_CudaView(self.heap_ptr, self.heap_bytes, self), device=f"cuda:{self.device}")
         self._bump = 0
+        self._lars_tables = {}     # device address of every validated LARS table -> (kind, rows, shard vectors or slots)
         # area of the barrier-free small-message all-reduce ("LL": the flag travels inside every 8-byte word)
         self.ll_words = int(os.environ.get("BNET_LL_WORDS", "8192"))          # 32 KiB of payload per rank and call
         area = int(self.lib.bnet_allreduce_ll_area_bytes(self.world, self.ll_words))
@@ -344,6 +384,83 @@ class SymmComm:
             self.h, self.offset_of(param), param.numel(), DT[param.dtype], C.c_void_p(scratch.data_ptr()),
             C.c_void_p(clip.data_ptr()), *scalars, *(C.c_void_p(s.data_ptr()) for s in state), channel, nblocks,
             self._stream(stream)), name)
+        self.launches += n
+
+    # ------------------------------------------------------------------ LARS (staged step: norm, trust, apply)
+    def lars_segments(self, table, shard_vecs: int, ntensors: int) -> torch.Tensor:
+        """Validate a bucket's LARS segment table on the host (``check_lars_segments``) and upload it: the kernels
+        accept only tables that went through here.  Returns the [nseg, 4] int32 device tensor."""
+        nslots = check_lars_segments(table, shard_vecs, ntensors)
+        t = torch.as_tensor(table, dtype=torch.int32).reshape(-1, 4).to(f"cuda:{self.device}").contiguous()
+        self._lars_tables[t.data_ptr()] = ("seg", t, shard_vecs, nslots, ntensors)
+        return t
+
+    def lars_tensors(self, table, nslots: int) -> torch.Tensor:
+        """Validate a LARS tensor table against `nslots` norm slots (``check_lars_tensors``) and upload it."""
+        check_lars_tensors(table, nslots)
+        t = torch.as_tensor(table, dtype=torch.int32).reshape(-1, 4).to(f"cuda:{self.device}").contiguous()
+        self._lars_tables[t.data_ptr()] = ("tensor", t, nslots, t.shape[0], t.shape[0])
+        return t
+
+    def _lars_table(self, t, kind, size):
+        rec = self._lars_tables.get(t.data_ptr())
+        if rec is None or rec[0] != kind or rec[1] is not t or rec[2] != size:
+            raise ValueError(f"LARS {kind} table was not validated for this shape: upload it with SymmComm.lars_{kind}s")
+        return rec
+
+    def fused_lars_norm(self, master: torch.Tensor, scratch: torch.Tensor, segs: torch.Tensor, slots: torch.Tensor,
+                        dtype: torch.dtype, nblocks: int = 0, stream=None):
+        """Per bucket, after stage 1: per chunk of each segment of ``segs`` (from ``lars_segments``), the float64 sums of
+        squares of this rank's fp32 ``master`` and ``scratch`` shard into the rows {sum w^2, sum g^2} of ``slots``
+        ([nslots, 2] float64).  ``dtype``: the parameters' dtype, which sets the elements per 16-byte vector."""
+        assert dtype in (torch.float32, torch.bfloat16)
+        assert master.is_cuda and master.dtype == torch.float32 and master.is_contiguous()
+        assert scratch.is_cuda and scratch.dtype == torch.float32 and scratch.is_contiguous() and scratch.numel() == master.numel()
+        per_vec = 16 // torch.empty((), dtype=dtype).element_size()
+        assert master.numel() % per_vec == 0
+        nslots = self._lars_table(segs, "seg", master.numel() // per_vec)[3]
+        assert slots.is_cuda and slots.dtype == torch.float64 and slots.is_contiguous() and tuple(slots.shape) == (nslots, 2)
+        n = self._chk(self.lib.bnet_fused_lars_norm(
+            self.h, master.numel() * self.world, DT[dtype], C.c_void_p(master.data_ptr()), C.c_void_p(scratch.data_ptr()),
+            C.c_void_p(segs.data_ptr()), segs.shape[0], C.c_void_p(slots.data_ptr()), nslots, nblocks, self._stream(stream)),
+            "fused_lars_norm")
+        self.launches += n
+
+    def fused_lars_trust(self, slots: torch.Tensor, tensors: torch.Tensor, xchg: torch.Tensor, clip: torch.Tensor,
+                         hp: torch.Tensor, scal: torch.Tensor, trust: torch.Tensor, channel: int = 0, stream=None):
+        """Once per step, after every norm launch: per tensor of ``tensors`` (from ``lars_tensors``), the norms over all
+        ranks (exchanged through the heap tensor ``xchg``, at least 2 * world * ntensors float64), the trust ratio into
+        ``trust`` ([ntensors] fp32) and the update scalars {grad scale, weight decay} into ``scal`` ([ntensors, 2] fp32).
+        ``clip``: the 4-float clip block (its clip_coef is used); ``hp``: the 8-float LARS block."""
+        T = tensors.shape[0]
+        self._lars_table(tensors, "tensor", slots.shape[0])
+        assert slots.is_cuda and slots.dtype == torch.float64 and slots.is_contiguous() and slots.dim() == 2 and slots.shape[1] == 2
+        assert xchg.numel() * xchg.element_size() >= 16 * self.world * T
+        assert clip.is_cuda and clip.dtype == torch.float32 and clip.numel() >= 4 and clip.is_contiguous()
+        assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= 8 and hp.is_contiguous()
+        assert scal.is_cuda and scal.dtype == torch.float32 and scal.is_contiguous() and tuple(scal.shape) == (T, 2)
+        assert trust.is_cuda and trust.dtype == torch.float32 and trust.is_contiguous() and trust.numel() == T
+        n = self._chk(self.lib.bnet_fused_lars_trust(
+            self.h, C.c_void_p(slots.data_ptr()), C.c_void_p(tensors.data_ptr()), T, self.offset_of(xchg),
+            C.c_void_p(clip.data_ptr()), C.c_void_p(hp.data_ptr()), C.c_void_p(scal.data_ptr()), C.c_void_p(trust.data_ptr()),
+            channel, self._stream(stream)), "fused_lars_trust")
+        self.launches += n
+
+    def fused_lars_apply(self, param: torch.Tensor, scratch: torch.Tensor, segs: torch.Tensor, scal: torch.Tensor,
+                         hp: torch.Tensor, master: torch.Tensor, mom: torch.Tensor, channel: int = 0, nblocks: int = 0,
+                         stream=None):
+        """Per bucket, after the trust kernel: the SGD step of ``fused_clip_apply_sgd`` from ``scratch``, with each
+        tensor's scalars from ``scal`` ([ntensors, 2], as many rows as the tensor count ``segs`` was validated for) and
+        lr and momentum from ``hp``, and the new ``param`` on every rank."""
+        assert scratch.dtype == torch.float32 and scratch.is_contiguous() and scratch.numel() * self.world == param.numel()
+        assert all(s.dtype == torch.float32 and s.is_contiguous() and s.numel() * self.world == param.numel() for s in (master, mom))
+        rec = self._lars_table(segs, "seg", param.numel() * param.element_size() // 16 // self.world)
+        assert scal.is_cuda and scal.dtype == torch.float32 and scal.is_contiguous() and tuple(scal.shape) == (rec[4], 2)
+        assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= 8 and hp.is_contiguous()
+        n = self._chk(self.lib.bnet_fused_lars_apply(
+            self.h, self.offset_of(param), param.numel(), DT[param.dtype], C.c_void_p(scratch.data_ptr()),
+            C.c_void_p(segs.data_ptr()), segs.shape[0], C.c_void_p(scal.data_ptr()), C.c_void_p(hp.data_ptr()),
+            C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), channel, nblocks, self._stream(stream)), "fused_lars_apply")
         self.launches += n
 
     # ------------------------------------------------------------------ collectives on ordinary tensors

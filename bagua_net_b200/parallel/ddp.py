@@ -18,7 +18,7 @@ from __future__ import annotations
 import torch
 import torch.distributed as dist
 
-from .comm import SymmComm
+from .comm import LARS_CHUNK, SymmComm
 
 
 def plan_buckets(numels, element_size: int, world: int, bucket_mb: float):
@@ -133,7 +133,38 @@ def direct_grads_self_check(device=None, group=None, steps: int = 3, make_model=
 
 
 # The fp32 tensors the fused kernel updates in every bucket's shard, master weights first; also their state-dict keys.
-_STATE_NAMES = {"sgd": ("master", "momentum"), "adamw": ("master", "exp_avg", "exp_avg_sq")}
+_STATE_NAMES = {"sgd": ("master", "momentum"), "adamw": ("master", "exp_avg", "exp_avg_sq"), "lars": ("master", "momentum")}
+
+
+def lars_segments(members, numels, start: int, numel: int, element_size: int, world: int, rank: int):
+    """The LARS segment table of one bucket on one rank: rows [vec0, nvec, tensor, slot0] (include/bnet/bnet_coll.h).
+
+    `members`: the bucket's [(parameter index, element offset in the flat buffer), ...] in offset order (plan_buckets);
+    `numels`: every parameter's element count; `start` / `numel`: the bucket's element range.  A segment is the part
+    of one tensor in this rank's shard, in 16-byte vectors relative to the shard.  Tensors start on 16-byte boundaries,
+    so no vector holds two tensors; the zero padding after a tensor joins the segment before it (padding at the start of
+    a shard joins the first segment, and a shard of padding alone becomes one segment of the bucket's last tensor).  The
+    rows cover the shard exactly once, and slot0 counts the LARS_CHUNK-vector chunks of the segments before."""
+    per_vec = 16 // element_size
+    shard = numel // world // per_vec                     # vectors in every rank's shard
+    lo = start + rank * shard * per_vec                   # the shard's element range
+    hi = lo + shard * per_vec
+    rows = []
+    for pi, off in members:
+        a, b = max(off, lo), min(off + numels[pi], hi)
+        if a < b:
+            rows.append([(a - lo) // per_vec, (b - lo + per_vec - 1) // per_vec, pi])
+    if not rows:
+        rows = [[0, shard, members[-1][0]]]
+    rows[0][0] = 0
+    for r, nxt in zip(rows, rows[1:]):
+        r[1] = nxt[0]                                     # [first, end) -> padding joins the segment before
+    rows[-1][1] = shard
+    table, slot = [], 0
+    for first, end, pi in rows:
+        table.append([first, end - first, pi, slot])
+        slot += (end - first + LARS_CHUNK - 1) // LARS_CHUNK
+    return table
 
 
 def _check_max_norm(v) -> float:
@@ -162,8 +193,15 @@ class _Bucket:
 
 class BnetDDP(torch.nn.Module):
     """Wraps ``module``; owns the optimizer, fused into the collective: ``optimizer="sgd"`` (SGD with momentum and L2
-    weight decay) or ``"adamw"`` (``torch.optim.AdamW`` with ``betas``, ``eps`` and decoupled ``weight_decay``;
-    AMSGrad and ``maximize`` are not offered).
+    weight decay), ``"adamw"`` (``torch.optim.AdamW`` with ``betas``, ``eps`` and decoupled ``weight_decay``;
+    AMSGrad and ``maximize`` are not offered) or ``"lars"``.
+
+    ``"lars"``: layer-wise adaptive rate scaling, as NVIDIA Apex's ``LARC(clip=False)`` around ``torch.optim.SGD``
+    (``momentum``, no dampening or Nesterov).  Every parameter tensor ``p`` with ``p.dim() > 1`` takes the trust ratio
+    ``t = trust_coefficient * |p| / (|g| + weight_decay * |p| + eps)`` of its whole-tensor norms (``t = 1`` and no weight
+    decay when either norm is 0, as in Apex) and steps with ``buf = momentum * buf + t * (g + weight_decay * p)``; biases and normalisation weights
+    (``p.dim() <= 1``) take ``g`` alone, as in MLPerf's ResNet-50.  ``g`` is the mean gradient (clipped first when
+    ``max_grad_norm`` is set).  The step is always staged; ``last_trust_ratios`` gives every tensor's ``t``.
 
     bucket_mb sizes buckets for launch latency and overlap (NVSwitch: no per-link bound).
 
@@ -186,16 +224,21 @@ class BnetDDP(torch.nn.Module):
                  bucket_mb: float = 64.0, comm: SymmComm | None = None, extra_heap_bytes: int = 64 << 20,
                  nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None,
-                 accumulation_steps: int = 1):
+                 accumulation_steps: int = 1, trust_coefficient: float = 0.001):
         super().__init__()
         if isinstance(accumulation_steps, bool) or not isinstance(accumulation_steps, int) or accumulation_steps < 1:
             raise ValueError(f"accumulation_steps must be an int >= 1 (got {accumulation_steps!r})")
         if max_grad_norm is not None:
             max_grad_norm = _check_max_norm(max_grad_norm)
-        if optimizer not in ("sgd", "adamw"):
-            raise ValueError(f"unknown optimizer {optimizer!r}: BnetDDP fuses 'sgd' or 'adamw'")
+        if optimizer not in ("sgd", "adamw", "lars"):
+            raise ValueError(f"unknown optimizer {optimizer!r}: BnetDDP fuses 'sgd', 'adamw' or 'lars'")
         if amsgrad or maximize:
-            raise ValueError("the fused AdamW offers neither amsgrad nor maximize")
+            raise ValueError("the fused optimizers offer neither amsgrad nor maximize")
+        if optimizer == "lars":
+            trust_coefficient, eps = float(trust_coefficient), float(eps)
+            if not trust_coefficient > 0.0 or not eps >= 0.0:
+                raise ValueError(f"LARS needs trust_coefficient > 0 and eps >= 0 (got {trust_coefficient}, {eps})")
+            self.trust_coefficient, self.eps = trust_coefficient, eps
         if optimizer == "adamw":
             if momentum is not None:
                 raise ValueError("AdamW has no momentum argument; use betas")
@@ -302,15 +345,20 @@ class BnetDDP(torch.nn.Module):
             shard = b.numel // comm.world
             master = b.param[comm.rank * shard:(comm.rank + 1) * shard].float().contiguous()
             b.state = (master,) + tuple(torch.zeros_like(master) for _ in _STATE_NAMES[optimizer][1:])
-        # AdamW always reads its hyper-parameters and step count from device memory (csrc/cuda/optim_body.cuh); SGD
-        # passes them as launch arguments until the first set_lr
-        self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev) if optimizer == "adamw" else None
+        # AdamW and LARS always read their hyper-parameters (and AdamW its step count) from device memory
+        # (csrc/cuda/optim_body.cuh); SGD passes them as launch arguments until the first set_lr
+        self._hp = None
+        if optimizer == "adamw":
+            self._hp = torch.tensor(self._adamw_hp(0), dtype=torch.float32, device=dev)
+        elif optimizer == "lars":
+            self._hp = torch.tensor(self._lars_hp(), dtype=torch.float32, device=dev)
         # the staged step (gradient clipping, gradient accumulation, or both): per bucket an fp32 scratch shard and a row
         # of per-CTA partial sums of squares.  Clipping adds one exchange area in the heap (same offset on every rank) and
         # the device block {max_norm, total_norm, clip_coef, reserved}; accumulation without clipping updates through the
         # constant block {inf, 0, 1, 0} instead (clip_coef exactly 1).
         self._clip = None
-        self._staged = max_grad_norm is not None or accumulation_steps > 1
+        # (LARS needs every tensor's whole norm before any of it is updated: always staged)
+        self._staged = max_grad_norm is not None or accumulation_steps > 1 or optimizer == "lars"
         if self._staged:
             from .comm import CLIP_ROW
 
@@ -320,9 +368,11 @@ class BnetDDP(torch.nn.Module):
         if max_grad_norm is not None:
             self._xchg = comm.alloc(comm.world, torch.float64)
             self._clip = torch.tensor([max_grad_norm, 0.0, 0.0, 0.0], dtype=torch.float32, device=dev)
-        elif accumulation_steps > 1:
+        elif self._staged:
             self._coef_one = torch.tensor([float("inf"), 0.0, 1.0, 0.0], dtype=torch.float32, device=dev)
         self.max_grad_norm = max_grad_norm
+        if optimizer == "lars":
+            self._lars_setup(params, plan, es, dev)
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad) for p in params]
@@ -407,11 +457,15 @@ class BnetDDP(torch.nn.Module):
                                       stream=self.comm_stream)
             coef = self._clip
         else:
+            coef = self._coef_one
+        if self.optimizer == "lars":
+            self._lars_update(coef)
+            return
+        if self._clip is None:
             # accumulation without clipping: only the barrier, and a coefficient of exactly 1.  (Not the coefficient
             # kernel at max_norm = inf: that turns a NaN norm into a NaN coefficient for every element, where an
             # unclipped torch step poisons only the NaN elements.)
             self.comm.barrier(channel=0, stream=self.comm_stream)
-            coef = self._coef_one
         for b in self.buckets:
             if not b.launched:
                 continue
@@ -423,6 +477,62 @@ class BnetDDP(torch.nn.Module):
                                                self.weight_decay, self._grad_scale, channel=0, nblocks=self.nblocks,
                                                stream=self.comm_stream, hp=self._hp)
             b.launched = False
+
+    # ------------------------------------------------------------------ LARS
+    def _lars_setup(self, params, plan, es, dev):
+        """Per bucket the validated segment table of this rank's shard and its norm slots; per tensor its slot range and
+        whether it is excluded; the exchange area in the heap, the update scalars and the trust ratios."""
+        comm, T = self.comm, len(params)
+        numels = [p.numel() for p in params]
+        tensors = [[0, 0, int(p.dim() <= 1), 0] for p in params]
+        self._lars_segs, self._lars_base, base = [], [], 0
+        for b, (start, numel, members) in zip(self.buckets, plan):
+            table = lars_segments(members, numels, start, numel, es, comm.world, comm.rank)
+            segs = comm.lars_segments(table, numel // comm.world * es // 16, T)
+            for vec0, nvec, pi, slot0 in table:
+                if tensors[pi][1]:
+                    raise AssertionError(f"tensor {pi} has two segments on one rank")
+                tensors[pi][:2] = [base + slot0, (nvec + LARS_CHUNK - 1) // LARS_CHUNK]
+            self._lars_segs.append(segs)
+            self._lars_base.append(base)
+            base += sum((nvec + LARS_CHUNK - 1) // LARS_CHUNK for _, nvec, _, _ in table)
+        self._lars_base.append(base)
+        self._lars_slots = torch.zeros(base, 2, dtype=torch.float64, device=dev)
+        self._lars_tensors = comm.lars_tensors(tensors, base)
+        self._lars_xchg = comm.alloc(2 * comm.world * T, torch.float64)
+        self._lars_scal = torch.zeros(T, 2, dtype=torch.float32, device=dev)
+        self._lars_trust = torch.ones(T, dtype=torch.float32, device=dev)
+
+    def _lars_update(self, coef):
+        """The LARS stages after the clipping coefficient: norms per launched bucket, the trust kernel (whose barrier is
+        the step's when there is no coefficient kernel), the update per launched bucket."""
+        st = self.comm_stream
+        for k, b in enumerate(self.buckets):
+            slots = self._lars_slots[self._lars_base[k]:self._lars_base[k + 1]]
+            if b.launched:
+                self.comm.fused_lars_norm(b.master, b.scratch, self._lars_segs[k], slots, self.dtype, nblocks=self.nblocks,
+                                          stream=st)
+            else:
+                with torch.cuda.stream(st):
+                    slots.zero_()                 # no gradient this step: its tensors' ratios read 1, and no update
+        self.comm.fused_lars_trust(self._lars_slots, self._lars_tensors, self._lars_xchg, coef, self._hp, self._lars_scal,
+                                   self._lars_trust, channel=0, stream=st)
+        for k, b in enumerate(self.buckets):
+            if not b.launched:
+                continue
+            self.comm.fused_lars_apply(b.param, b.scratch, self._lars_segs[k], self._lars_scal, self._hp, *b.state, channel=0,
+                                       nblocks=self.nblocks, stream=st)
+            b.launched = False
+
+    def _lars_hp(self) -> list:
+        return [self.lr, self.momentum, self.weight_decay, self._grad_scale, self.trust_coefficient, self.eps, 0.0, 0.0]
+
+    @property
+    def last_trust_ratios(self) -> torch.Tensor | None:
+        """LARS: the trust ratio of every trainable parameter of the most recent step, in ``module.parameters()`` order
+        (1 for the excluded ``p.dim() <= 1`` tensors and for tensors without a gradient in the step), as a new fp32
+        tensor on the device.  ``None`` for the other optimizers."""
+        return None if self.optimizer != "lars" else self._lars_trust.clone()
 
     # ------------------------------------------------------------------ user API
     def forward(self, *args, **kwargs):
@@ -616,6 +726,9 @@ class BnetDDP(torch.nn.Module):
         if self.optimizer == "adamw":
             head = {"optimizer": "adamw", "lr": self.lr, "betas": self.betas, "eps": self.eps,
                     "weight_decay": self.weight_decay, "step": int(self._hp[self._HP_STEP].item())}
+        elif self.optimizer == "lars":
+            head = {"optimizer": "lars", "lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay,
+                    "trust_coefficient": self.trust_coefficient, "eps": self.eps}
         else:
             head = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
         names = _STATE_NAMES[self.optimizer]
@@ -638,6 +751,11 @@ class BnetDDP(torch.nn.Module):
             self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
             self.betas = tuple(state["betas"])
             self._hp.copy_(torch.tensor(self._adamw_hp(state["step"]), dtype=torch.float32))
+            return
+        if self.optimizer == "lars":
+            self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
+            self.trust_coefficient, self.eps = state["trust_coefficient"], state["eps"]
+            self._hp.copy_(torch.tensor(self._lars_hp(), dtype=torch.float32))
             return
         self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
         if self._hp is not None:
@@ -665,7 +783,8 @@ class BnetDDP(torch.nn.Module):
         """Learning-rate schedule hook.  From the first call on, the fused optimizer kernels read {lr, momentum,
         weight decay, 1/world} from a 4-float device tensor instead of baked-in launch arguments, so a captured CUDA
         graph is re-captured once (here) and then follows the schedule with one tiny host→device write per change.
-        AdamW reads its hyper-parameters from device memory from the start (no re-capture at all) and has no momentum."""
+        AdamW and LARS read theirs from device memory from the start (no re-capture at all); AdamW has no momentum, and
+        LARS's block also holds its trust coefficient and eps, fixed at construction."""
         if self.optimizer == "adamw":
             if momentum is not None:
                 raise ValueError("AdamW has no momentum; its betas are fixed at construction")
@@ -681,6 +800,9 @@ class BnetDDP(torch.nn.Module):
         if weight_decay is not None:
             self.weight_decay = float(weight_decay)
         vals = [self.lr, self.momentum, self.weight_decay, self._grad_scale]
+        if self.optimizer == "lars":           # (the block has been in device memory since construction)
+            self._hp.copy_(torch.tensor(self._lars_hp(), dtype=torch.float32))
+            return
         if self._hp is None:
             self._hp = torch.tensor(vals, dtype=torch.float32, device=self.flat_param.device)
             self._graph = None

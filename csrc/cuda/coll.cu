@@ -507,6 +507,34 @@ struct ScratchGrad {
   const float* g;
   float coef;
 };
+// LARS: the scratch as in ScratchGrad, but every vector scaled by its own tensor's gradient scale (which folds in the
+// clipping coefficient and the trust ratio) and decayed by its tensor's weight decay: the pair scal[tensor], where the
+// tensor is the one of the segment (BnetLarsSeg, sorted by vec0) that holds the shard vector.
+struct LarsGrad {
+  const float* g;
+  const int4* seg;   // {vec0, nvec, tensor, slot0}
+  int nseg;
+  const float2* scal;
+};
+// The update scalars of shard vector v's tensor, found by a binary search over the sorted segment starts, in L1-resident table entries.
+__device__ __forceinline__ float2 lars_vec_scalars(const LarsGrad& s, size_t v) {
+  int lo = 0, hi = s.nseg - 1;
+  while (lo < hi) {
+    const int m = (lo + hi + 1) >> 1;
+    if ((size_t)__ldg(&s.seg[m].x) <= v) lo = m;
+    else hi = m - 1;
+  }
+  return __ldg(s.scal + __ldg(&s.seg[lo].z));
+}
+// SGD with momentum whose gradient scale and weight decay come per vector from LarsGrad (lr and momentum are the step's).
+// U vectors per batch: the bf16 variants take one, as AdamW does, because the table search on top of two vectors'
+// loads spills at the 64-register cap of two 512-thread CTAs per SM.
+template <int U>
+struct LarsOpt {
+  static constexpr int kStates = 2;   // master, momentum
+  static constexpr int kU = U;
+  float lr, mu;
+};
 
 // One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch reductions / peer loads or the
 // fp32 scratch, the fp32 state) are issued before any dependent math so that U*(1 + S*E/4) requests per thread are in
@@ -518,6 +546,7 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, const G& src, size
   constexpr int Q = E / 4;
   constexpr int S = Opt::kStates;
   constexpr bool kHeap = std::is_same<G, HeapGrad>::value;
+  constexpr bool kLars = std::is_same<G, LarsGrad>::value;
   int4 gv[U];
   float4 sm[U][S][Q];
   float gp2p[(MODE == 2) ? U : 1][8];
@@ -540,8 +569,17 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, const G& src, size
 #pragma unroll
   for (int u = 0; u < U; u++) {
     float g[8], st[S][8];
+    [[maybe_unused]] float2 sc;
     if constexpr (kHeap) {
       fused_grad_get<DT, MODE>(gv[u], gp2p[(MODE == 2) ? u : 0], g);
+    } else if constexpr (kLars) {
+      // (the table search runs while the batch's later loads are still in flight)
+      sc = lars_vec_scalars(src, i + u * stride);
+#pragma unroll
+      for (int q = 0; q < Q; q++) {
+        g[4 * q] = gs[u][q].x * sc.x; g[4 * q + 1] = gs[u][q].y * sc.x;
+        g[4 * q + 2] = gs[u][q].z * sc.x; g[4 * q + 3] = gs[u][q].w * sc.x;
+      }
     } else {
 #pragma unroll
       for (int q = 0; q < Q; q++) {
@@ -555,8 +593,15 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, const G& src, size
       for (int s = 0; s < S; s++) {
         st[s][4 * q] = sm[u][s][q].x; st[s][4 * q + 1] = sm[u][s][q].y; st[s][4 * q + 2] = sm[u][s][q].z; st[s][4 * q + 3] = sm[u][s][q].w;
       }
+    if constexpr (kLars) {
+      // per-element sgd_update with the vector's scalars: g already carries its gradient scale
+      const SgdOpt o{opt.lr, opt.mu, sc.y, 1.0f};
 #pragma unroll
-    for (int k = 0; k < E; k++) opt.update(g[k], st, k);
+      for (int k = 0; k < E; k++) o.update(g[k], st, k);
+    } else {
+#pragma unroll
+      for (int k = 0; k < E; k++) opt.update(g[k], st, k);
+    }
 #pragma unroll
     for (int q = 0; q < Q; q++)
 #pragma unroll
@@ -766,6 +811,132 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_adamw_kernel(Coll
   float* const state[3] = {master, exp_avg, exp_avg_sq};
   fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, 0,
                        chan);
+}
+
+// ------------------------------------------------------------------ LARS: per-tensor trust ratios in the staged step
+// Sums of two doubles per thread over a kThreads-thread CTA in a fixed order (cta_sum's butterfly, then the warps in
+// order), valid in thread 0.  Unlike cta_sum it may be called repeatedly: the leading barrier keeps a call's writes of
+// the warp sums behind the previous call's reads.
+__device__ __forceinline__ double2 cta_sum2(double a, double b) {
+  __shared__ double2 warp_sums[kThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = make_double2(a, b);
+  __syncthreads();
+  double2 s = make_double2(0.0, 0.0);
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kThreads / 32; w++) {
+      s.x += warp_sums[w].x;
+      s.y += warp_sums[w].y;
+    }
+  return s;
+}
+
+// Per bucket, after stage 1: the sums of squares of this rank's fp32 master and scratch shards per chunk of
+// BNET_LARS_CHUNK vectors of each segment, into the chunk's slot {sum w^2, sum g^2}.  A CTA takes whole chunks (grid
+// stride over the bucket's `nslots` slots) and finds a slot's segment by a binary search over the segments' slot0.  Each
+// chunk is summed the same way whichever CTA takes it, so the bits depend neither on the grid nor on a repeat, and no
+// atomics are needed.  `q`: float4s per vector (1 for fp32 parameters, 2 for bf16).
+__global__ void __launch_bounds__(kThreads) bnet_lars_norm_kernel(const float4* __restrict__ master, const float4* __restrict__ scratch,
+                                                                 const int4* __restrict__ seg, int nseg, int q,
+                                                                 double2* __restrict__ slots, int nslots) {
+  for (int j = blockIdx.x; j < nslots; j += gridDim.x) {
+    int lo = 0, hi = nseg - 1;
+    while (lo < hi) {
+      const int m = (lo + hi + 1) >> 1;
+      if (__ldg(&seg[m].w) <= j) lo = m;
+      else hi = m - 1;
+    }
+    const int4 s = __ldg(seg + lo);
+    const size_t v0 = (size_t)s.x + (size_t)(j - s.w) * BNET_LARS_CHUNK;
+    const size_t v1 = (size_t)s.x + (size_t)s.y < v0 + BNET_LARS_CHUNK ? (size_t)s.x + (size_t)s.y : v0 + BNET_LARS_CHUNK;
+    double w2 = 0.0, g2 = 0.0;
+#pragma unroll 4
+    for (size_t f = v0 * q + threadIdx.x; f < v1 * q; f += kThreads) {
+      const float4 w = ptx::ld_na_f4(master + f);
+      const float4 g = ptx::ld_na_f4(scratch + f);
+      w2 = fma((double)w.x, (double)w.x, w2); w2 = fma((double)w.y, (double)w.y, w2);
+      w2 = fma((double)w.z, (double)w.z, w2); w2 = fma((double)w.w, (double)w.w, w2);
+      g2 = fma((double)g.x, (double)g.x, g2); g2 = fma((double)g.y, (double)g.y, g2);
+      g2 = fma((double)g.z, (double)g.z, g2); g2 = fma((double)g.w, (double)g.w, g2);
+    }
+    const double2 r = cta_sum2(w2, g2);
+    if (threadIdx.x == 0) slots[j] = r;
+  }
+}
+
+// Once per step, one CTA, after every bucket's norm launch: per tensor (one warp each, lanes over its slots, then a
+// fixed butterfly) this rank's {sum w^2, sum g^2}, written into every rank's exchange area ([world][2][ntensors] doubles
+// at heap byte offset `xoff`); after a rank barrier, per tensor (one thread each) the sums over the ranks in rank order
+// 0..world-1 -- the same bits on every rank -- and the trust ratio and update scalars.  The second rank barrier lets the
+// exchange area be reused next step, as in bnet_clip_coef_kernel; with one rank a CTA barrier stands for the first.
+// Without clipping, the first barrier is the staged step's barrier before its update stage.
+__global__ void __launch_bounds__(kThreads) bnet_lars_trust_kernel(CollDev d, const double2* __restrict__ slots,
+                                                                  const int4* __restrict__ tens, int ntensors, size_t xoff,
+                                                                  const float* __restrict__ clip, const float* __restrict__ hp,
+                                                                  float2* __restrict__ scal, float* __restrict__ trust, int chan) {
+  const int lane = threadIdx.x & 31;
+  const size_t T = (size_t)ntensors;
+  for (int j = threadIdx.x >> 5; j < ntensors; j += kThreads / 32) {
+    const int4 t = tens[j];
+    double w2 = 0.0, g2 = 0.0;
+    for (int k = lane; k < t.y; k += 32) {
+      const double2 s = slots[t.x + k];
+      w2 += s.x;
+      g2 += s.y;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      w2 += __shfl_xor_sync(0xffffffffu, w2, o);
+      g2 += __shfl_xor_sync(0xffffffffu, g2, o);
+    }
+    if (lane == 0)
+      for (int p = 0; p < d.world; p++) {
+        volatile double* x = reinterpret_cast<volatile double*>(d.heap[p] + xoff) + 2 * T * d.rank;
+        x[j] = w2;
+        x[T + j] = g2;
+      }
+  }
+  if (d.world > 1) {
+    __threadfence_system();
+    rank_barrier(d, chan);
+  } else {
+    __syncthreads();
+  }
+  const float coef = clip[optim::kClipCoef];
+  const float gscale = hp[optim::kLarsGradScale], wd = hp[optim::kLarsWeightDecay];
+  const float eta = hp[optim::kLarsEta], eps = hp[optim::kLarsEps];
+  const float gs = gscale * coef;
+  const volatile double* x = reinterpret_cast<const volatile double*>(d.heap[d.rank] + xoff);
+  for (int j = threadIdx.x; j < ntensors; j += kThreads) {
+    double w2 = x[j], g2 = x[T + j];
+    for (int p = 1; p < d.world; p++) {
+      w2 += x[2 * T * p + j];
+      g2 += x[2 * T * p + T + j];
+    }
+    const float wn = (float)sqrt(w2);
+    const float gn = (float)(sqrt(g2) * (double)gscale * (double)coef);
+    const optim::LarsScalars ls = optim::lars_scalars(eta, eps, wd, gs, wn, gn, tens[j].z != 0);
+    scal[j] = make_float2(ls.gscale, ls.wd);
+    trust[j] = ls.t;
+  }
+  if (d.world > 1) rank_barrier(d, chan);
+}
+
+// Per bucket, after the trust kernel: fused_step from the scratch with each vector's tensor's scalars (LarsGrad), then
+// the parameter broadcast and the closing barrier, as bnet_clip_apply_sgd_kernel.
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_lars_apply_kernel(CollDev d, size_t poff, size_t nvec, const float* __restrict__ scratch,
+                                                                  const int4* __restrict__ seg, int nseg, const float2* __restrict__ scal,
+                                                                  const float* __restrict__ hp, float* __restrict__ master,
+                                                                  float* __restrict__ mom, int chan) {
+  float* const state[2] = {master, mom};
+  fused_step<DT, MODE>(d, LarsGrad{scratch, seg, nseg, scal}, poff, nvec, LarsOpt<DT == BNET_BF16 ? 1 : 2>{hp[optim::kLarsLr], hp[optim::kLarsMomentum]},
+                       state, 0, chan);
 }
 
 // ------------------------------------------------------------------ multi-tensor pack + cast (K5)
@@ -1445,6 +1616,61 @@ BNET_API int bnet_fused_clip_apply_adamw(BnetColl* c, size_t param_off, size_t c
                      stream, f) < 0)
     return -1;
   return run_fused_kernel<ClipAdamWKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, hp_dev, master, exp_avg, exp_avg_sq, channel);
+}
+
+// ---- LARS: norm, trust and apply stages (the tables themselves are validated by the caller before upload)
+struct LarsApplyKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_lars_apply_kernel<DT, MODE>;
+};
+static_assert(sizeof(BnetLarsSeg) == sizeof(int4) && sizeof(BnetLarsTensor) == sizeof(int4), "LARS tables are int4 rows");
+
+static int lars_seg_check(const BnetLarsSeg* segs, int nseg) {
+  if (nseg < 1 || !segs || ((uintptr_t)segs & 15)) return fail("LARS segment table needs >= 1 row, 16-byte aligned");
+  return 0;
+}
+
+BNET_API int bnet_fused_lars_norm(BnetColl* c, size_t count, int dtype, const float* master, const float* scratch,
+                                  const BnetLarsSeg* segs, int nseg, double* slots, int nslots, int nblocks, void* stream) {
+  if (dtype != BNET_F32 && dtype != BNET_BF16) return fail("LARS norm supports f32 and bf16");
+  if ((count * elsize(dtype)) % (16 * (size_t)c->world)) return fail("LARS norm needs bytes%%(16*world)==0");
+  if (((uintptr_t)master | (uintptr_t)scratch | (uintptr_t)slots) & 15) return fail("LARS norm buffers must be 16-byte aligned");
+  if (lars_seg_check(segs, nseg) < 0) return -1;
+  if (nslots < 1) return fail("LARS norm needs >= 1 slot");
+  int nb = nblocks > 0 ? nblocks : (int)env_int("COLL_BLOCKS_SINGLE", 264);
+  if (nb > nslots) nb = nslots;
+  if (nb > BNET_COLL_MAX_BLOCKS) nb = BNET_COLL_MAX_BLOCKS;
+  return launch(bnet_lars_norm_kernel, nb, kThreads, (cudaStream_t)stream, reinterpret_cast<const float4*>(master),
+                reinterpret_cast<const float4*>(scratch), reinterpret_cast<const int4*>(segs), nseg, dtype == BNET_BF16 ? 2 : 1,
+                reinterpret_cast<double2*>(slots), nslots);
+}
+
+BNET_API int bnet_fused_lars_trust(BnetColl* c, const double* slots, const BnetLarsTensor* tensors, int ntensors, size_t xchg_off,
+                                   const float* clip, const float* hp, float* scal, float* trust, int channel, void* stream) {
+  if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
+  if (ntensors < 1 || !tensors || ((uintptr_t)tensors & 15)) return fail("LARS tensor table needs >= 1 row, 16-byte aligned");
+  if (!slots || ((uintptr_t)slots & 15)) return fail("LARS slots must be a 16-byte aligned device pointer");
+  if (clip_block_check(clip) < 0) return -1;
+  if (!hp || ((uintptr_t)hp & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (!scal || ((uintptr_t)scal & 7) || !trust || ((uintptr_t)trust & 3)) return fail("LARS outputs must be aligned device pointers");
+  if (xchg_off % 16 || xchg_off + 2 * (size_t)c->world * ntensors * sizeof(double) > c->alloc_bytes - kPadBytes)
+    return fail("LARS exchange area must be 16-byte aligned and inside the heap");
+  refresh_devp(c);
+  return launch(bnet_lars_trust_kernel, 1, kThreads, (cudaStream_t)stream, c->devp, reinterpret_cast<const double2*>(slots),
+                reinterpret_cast<const int4*>(tensors), ntensors, kPadBytes + xchg_off, clip, hp, reinterpret_cast<float2*>(scal),
+                trust, channel);
+}
+
+BNET_API int bnet_fused_lars_apply(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch, const BnetLarsSeg* segs,
+                                   int nseg, const float* scal, const float* hp, float* master, float* mom_buf, int channel, int nblocks,
+                                   void* stream) {
+  if (!hp || ((uintptr_t)hp & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (lars_seg_check(segs, nseg) < 0) return -1;
+  if (!scal || ((uintptr_t)scal & 7)) return fail("LARS scalars must be an 8-byte aligned device pointer");
+  FusedLaunch f;
+  if (fused_prologue(c, "LARS", param_off, param_off, count, dtype, channel, {scratch, master, mom_buf}, nblocks, stream, f) < 0)
+    return -1;
+  return run_fused_kernel<LarsApplyKernel>(c, dtype, f, f.poff, f.nvec, scratch, reinterpret_cast<const int4*>(segs), nseg,
+                                           reinterpret_cast<const float2*>(scal), hp, master, mom_buf, channel);
 }
 
 BNET_API int bnet_pack_cast(const BnetPackItem* items_dev, int n, void* dst, int src_dtype, int dst_dtype, float scale,

@@ -1,5 +1,6 @@
 // Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu): sgd_update for
-// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, and clip_coef for the clipped step.
+// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, clip_coef for the clipped step, and lars_trust /
+// lars_scalars for the LARS step.
 //
 // The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
 // kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks SGD and AdamW against long-double
@@ -90,6 +91,32 @@ BNET_OPT_HD float clip_coef(float max_norm, float total_norm) {
 // Device block of the clipped step (separate from the optimizers' hyper-parameter blocks): 4 floats, 16-byte aligned.
 // max_norm is written by the host; the norm kernel writes total_norm (before clipping) and clip_coef every step.
 enum { kClipMaxNorm = 0, kClipTotalNorm, kClipCoef, kClipReserved, kClipWords };
+
+// LARS trust ratio of one tensor, as NVIDIA Apex's LARC (clip=False) computes it from the tensor's weight norm wn and
+// gradient norm gn:  t = eta * wn / (gn + wd * wn + eps),  and t = 1 when wn == 0 or gn == 0.  The tests are == 0 as
+// in Apex, so a NaN norm gives a NaN ratio (the tensor is poisoned, as in the reference) and gn = inf gives t = 0.
+BNET_OPT_HD float lars_trust(float eta, float eps, float wd, float wn, float gn) {
+  if (wn == 0.0f || gn == 0.0f) return 1.0f;
+  return eta * wn / (fmaf(wd, wn, gn) + eps);
+}
+
+// One tensor's LARS step as update scalars for sgd_update (with the tensor's gradient already summed over ranks):
+// gscale = grad_scale * clip_coef * t and wd = weight_decay * t, so that buf = mu*buf + t*(g + wd*p) up to rounding.
+// Excluded tensors (biases, normalisation weights) take t = 1 and no weight decay.  When either norm is 0, Apex's LARC
+// leaves the gradient alone -- t = 1 and no weight decay either -- and so does this.
+struct LarsScalars {
+  float t, gscale, wd;
+};
+BNET_OPT_HD LarsScalars lars_scalars(float eta, float eps, float wd, float gs, float wn, float gn, bool excluded) {
+  if (excluded || wn == 0.0f || gn == 0.0f) return {1.0f, gs, 0.0f};
+  const float t = lars_trust(eta, eps, wd, wn, gn);
+  return {t, gs * t, wd * t};
+}
+
+// Hyper-parameter block of the LARS step: 8 floats of device memory, 16-byte aligned, read when the kernels run.
+// The first four are the SGD block's {lr, momentum, weight_decay, grad_scale}.
+enum { kLarsLr = 0, kLarsMomentum, kLarsWeightDecay, kLarsGradScale, kLarsEta, kLarsEps, kLarsReserved0, kLarsReserved1,
+       kLarsWords };
 
 }  // namespace optim
 }  // namespace bnet

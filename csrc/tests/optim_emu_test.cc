@@ -1,6 +1,7 @@
 // CPU test of the fused optimizer updates: compiles the per-element bodies of csrc/cuda/optim_body.cuh (what
 // bnet_fused_adamw_kernel and bnet_fused_sgd_kernel inline) with g++ and compares them with a long-double AdamW and SGD
-// fed the same fp32 inputs and the same fp32 hyper-parameters.  The SGD part and its bound are further down.
+// fed the same fp32 inputs and the same fp32 hyper-parameters.  The SGD part and its bound are further down, and so is
+// the LARS trust ratio (lars_trust / lars_scalars).
 //
 // AdamW:
 // Bound (u = 2^-24, F = 4 * 2^-149 for results in the subnormal range).  With M = b1|m| + (1-b1)|g|,
@@ -237,12 +238,75 @@ static void sgd_checks() {
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------- LARS
+// lars_trust against long double on the same fp32 inputs: t = eta*wn / ((gn + wd*wn) + eps) takes four roundings
+// (product, fma, add, divide) of non-negative terms, so |t - T| <= 4.5u T (+ F).  The special cases follow Apex's
+// LARC: t = 1 when a norm is exactly 0, NaN from a NaN norm, 0 from an infinite gradient norm.  lars_scalars must give
+// {t, gs*t, wd*t}, or {1, gs, 0} for excluded tensors and zero norms.
+static double l_worst = 0.0;
+
+static LD lars_ref(float eta, float eps, float wd, float wn, float gn) {
+  return (LD)eta * wn / ((LD)gn + (LD)wd * wn + (LD)eps);
+}
+
+static void lars_checks() {
+  const float etas[] = {1e-3f, 0.02f, 1.f};
+  const float epss[] = {0.f, 1e-8f, 1e-3f};
+  const float wds[] = {0.f, 5e-5f, 1e-4f, 0.1f};
+  for (const float eta : etas)
+    for (const float eps : epss)
+      for (const float wd : wds)
+        for (int i = 0; i < 4000; i++) {
+          // norms from 2^-60 to 2^40: tiny and huge gradients, layers of any size
+          const float wn = ldexpf(0.5f + urand(), (int)(urand() * 100.f) - 60);
+          const float gn = ldexpf(0.5f + urand(), (int)(urand() * 100.f) - 60);
+          const float t = lars_trust(eta, eps, wd, wn, gn);
+          const LD T = lars_ref(eta, eps, wd, wn, gn);
+          const LD bound = 4.5L * kU * fabsl(T) + kF;
+          const LD err = fabsl((LD)t - T);
+          CHECK(isfinite(t) && err <= bound, "lars_trust(%g, %g, %g, %g, %g) = %.9g, reference %.12Lg", eta, eps, wd, wn, gn, t, T);
+          if ((double)(err / bound) > l_worst) l_worst = (double)(err / bound);
+          const float gs = 0.125f * (0.5f + urand());
+          const LarsScalars s = lars_scalars(eta, eps, wd, gs, wn, gn, false);
+          CHECK(s.t == t && s.gscale == gs * t && s.wd == wd * t, "lars_scalars != {t, gs*t, wd*t}");
+          const LarsScalars x = lars_scalars(eta, eps, wd, gs, wn, gn, true);
+          CHECK(x.t == 1.f && x.gscale == gs && x.wd == 0.f, "excluded tensor: {%g, %g, %g}", x.t, x.gscale, x.wd);
+        }
+  // the special cases of Apex's LARC (clip=False)
+  const float eta = 1e-3f, eps = 1e-8f, wd = 1e-4f;
+  CHECK(lars_trust(eta, eps, wd, 0.f, 3.f) == 1.f, "wn == 0 -> 1");
+  CHECK(lars_trust(eta, eps, wd, 3.f, 0.f) == 1.f, "gn == 0 -> 1");
+  CHECK(lars_trust(eta, eps, wd, 0.f, 0.f) == 1.f, "both 0 -> 1");
+  CHECK(lars_trust(eta, eps, wd, -0.f, 3.f) == 1.f, "wn == -0 -> 1");
+  CHECK(isnan(lars_trust(eta, eps, wd, NAN, 3.f)), "NaN wn -> NaN");
+  CHECK(isnan(lars_trust(eta, eps, wd, 3.f, NAN)), "NaN gn -> NaN");
+  CHECK(isnan(lars_trust(eta, eps, wd, NAN, 0.f)) == false && lars_trust(eta, eps, wd, NAN, 0.f) == 1.f,
+        "gn == 0 wins over a NaN wn, as Apex's 'and'");
+  CHECK(lars_trust(eta, eps, wd, 3.f, INFINITY) == 0.f, "gn = inf -> 0");
+  CHECK(isnan(lars_trust(eta, eps, wd, INFINITY, 3.f)), "wn = inf with wd > 0 -> inf / inf = NaN");
+  CHECK(isnan(lars_trust(eta, eps, 0.f, INFINITY, 3.f)), "wn = inf with wd = 0 -> NaN (inf * 0 in the denominator, as Apex)");
+  CHECK(lars_trust(eta, 0.f, 0.f, 2.f, 4.f) == eta * 0.5f, "eps = wd = 0: eta * wn / gn");
+  const LarsScalars z = lars_scalars(eta, eps, wd, 0.25f, 3.f, 0.f, false);
+  CHECK(z.t == 1.f && z.gscale == 0.25f && z.wd == 0.f, "zero gradient norm: no weight decay, as in Apex");
+  const LarsScalars zw = lars_scalars(eta, eps, wd, 0.25f, 0.f, 2.f, false);
+  CHECK(zw.t == 1.f && zw.gscale == 0.25f && zw.wd == 0.f, "zero weight norm: {1, gs, 0}");
+  const LarsScalars n = lars_scalars(eta, eps, wd, 0.25f, 3.f, NAN, false);
+  CHECK(isnan(n.t) && isnan(n.gscale) && isnan(n.wd), "NaN gradient norm poisons the tensor");
+  const LarsScalars f = lars_scalars(eta, eps, wd, 0.25f, 3.f, INFINITY, false);
+  CHECK(f.t == 0.f && f.gscale == 0.f && f.wd == 0.f, "infinite gradient norm: t = 0");
+  const LarsScalars e = lars_scalars(eta, eps, wd, NAN, 3.f, 2.f, true);
+  CHECK(e.t == 1.f && isnan(e.gscale) && e.wd == 0.f, "excluded tensor keeps a NaN clip coefficient in its scale");
+}
+
 int main() {
+  lars_checks();
+  const int lars = g_checks;
+  printf("optim_emu_test: lars %d checks, worst error/bound %.3f\n", lars, l_worst);
   adamw_checks();
-  const int adamw = g_checks;
+  const int adamw = g_checks - lars;
   printf("optim_emu_test: adamw %d checks, worst error/bound %.3f\n", adamw, g_worst);
   sgd_checks();
-  printf("optim_emu_test: sgd %d checks, worst error/bound %.3f\n", g_checks - adamw, s_worst);
+  printf("optim_emu_test: sgd %d checks, worst error/bound %.3f\n", g_checks - adamw - lars, s_worst);
   printf("optim_emu_test: %d checks, %d failures\n", g_checks, g_fail);
   if (g_fail) return 1;
   printf("optim_emu_test: ok\n");

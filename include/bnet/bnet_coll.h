@@ -134,6 +134,47 @@ int bnet_fused_clip_apply_adamw(BnetColl* c, size_t param_off, size_t count, int
                                 const float* hp_dev, float* master, float* exp_avg, float* exp_avg_sq, int channel, int nblocks,
                                 void* stream);
 
+/* LARS (layer-wise adaptive rate scaling, NVIDIA Apex LARC with clip=False, then SGD with momentum) in the staged step.
+ * Stage 1 is bnet_fused_clip_reduce_norm / bnet_fused_accum_reduce_norm as above.  Each parameter tensor's update takes a
+ * trust ratio from the norms of the WHOLE tensor, so three more launches follow, on the same stream:
+ *
+ * A segment is the part of one parameter tensor that lies in this rank's shard of a bucket: `nvec` 16-byte vectors from
+ * shard vector `vec0` (every tensor starts on a 16-byte boundary, so a vector belongs to one tensor; zero padding
+ * vectors may belong to either neighbouring segment).  A bucket's table lists its segments sorted by vec0 and covers
+ * the shard exactly once.  Each segment is cut into chunks of BNET_LARS_CHUNK vectors, and chunk k of a segment owns
+ * norm slot `slot0 + k` (slot0 is a running count over the bucket's segments).  The caller validates the tables before
+ * it uploads them: the kernels trust them. */
+#define BNET_LARS_CHUNK 4096
+typedef struct {
+  int32_t vec0, nvec, tensor, slot0;
+} BnetLarsSeg;
+/* Per tensor, for the trust kernel: its norm slots [slot0, slot0 + nslots) in the slot array of all buckets (nslots = 0
+ * when no part of it is in this rank's shards); `excluded` != 0 for tensors that take no trust ratio or weight decay. */
+typedef struct {
+  int32_t slot0, nslots, excluded, reserved;
+} BnetLarsTensor;
+/* Per bucket, once per step after stage 1: for each chunk of each segment, the sums of squares (in double, fixed order,
+ * no atomics: the bits depend on neither the grid nor the repeat) of this rank's fp32 `master` and `scratch` shard
+ * (count/world floats each) into slots[2 * slot] = sum w^2 and slots[2 * slot + 1] = sum g^2.  Rank-local. */
+int bnet_fused_lars_norm(BnetColl* c, size_t count, int dtype, const float* master, const float* scratch,
+                         const BnetLarsSeg* segs, int nseg, double* slots, int nslots, int nblocks, void* stream);
+/* Once per step, after every norm launch (and after bnet_fused_clip_coef when clipping; its barrier then is the
+ * step's): per tensor, sum its slots, exchange the per-rank (sum w^2, sum g^2) through 2 * world * ntensors doubles at
+ * heap byte offset `xchg_off` (16-byte aligned, same on every rank, used by nothing else) and add them in rank order, so
+ * every rank gets the same bits; then wn = sqrt(w^2), gn = sqrt(g^2) * grad_scale * clip_coef,
+ * t = lars_trust(eta, eps, wd, wn, gn) (csrc/cuda/optim_body.cuh), and the tensor's update scalars
+ * scal[2j] = grad_scale * clip_coef * t, scal[2j + 1] = wd * t (excluded: grad_scale * clip_coef and 0, t = 1), and
+ * trust[j] = t.  `clip`: the 4-float clip block (clip_coef read from it); `hp`: the 8-float LARS block
+ * {lr, momentum, weight_decay, grad_scale, trust_coefficient, eps, reserved, reserved}.  One CTA, two rank barriers. */
+int bnet_fused_lars_trust(BnetColl* c, const double* slots, const BnetLarsTensor* tensors, int ntensors, size_t xchg_off,
+                          const float* clip, const float* hp, float* scal, float* trust, int channel, void* stream);
+/* Per bucket after the trust kernel: the SGD update of bnet_fused_clip_apply_sgd_hp from `scratch`, with every vector's
+ * gradient scale and weight decay taken from its tensor's scal pair (lr and momentum from hp), then the parameter
+ * broadcast and a closing barrier. */
+int bnet_fused_lars_apply(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch, const BnetLarsSeg* segs,
+                          int nseg, const float* scal, const float* hp, float* master, float* mom_buf, int channel, int nblocks,
+                          void* stream);
+
 /* Multi-tensor pack+cast into the heap (K5): n tensors described on the device. */
 typedef struct {
   const void* src;

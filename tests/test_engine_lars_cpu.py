@@ -1,0 +1,310 @@
+"""BnetDDP(optimizer="lars")'s HOST logic on the CPU: the segment tables (a pure function, at world 1, 2, 3 and 8), the
+staged step's launch order, the update against a float64 LARC + torch.optim.SGD reference (with and without clipping,
+with accumulation, both memory formats, adopted and accumulated gradients), set_lr mid-run, the state dict, a bucket
+without gradient and every rejected argument.  The comm below does the stages in plain PyTorch with the kernels'
+arithmetic; the kernels are covered on the GPU by tests/test_fused_lars.py."""
+import copy
+import math
+
+import pytest
+import torch
+from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import small_model as _model
+
+from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_lars_segments, check_lars_tensors
+from bagua_net_b200.parallel.ddp import BnetDDP, lars_segments, plan_buckets
+
+
+class LarsComm(FakeComm):
+    """FakeComm plus the staged step and the three LARS stages; `log` lists every call in order."""
+
+    def __init__(self):
+        super().__init__()
+        self.log = []
+
+    def _stage1(self, kind, grad, scratch, partial, add):
+        assert partial.numel() == CLIP_ROW
+        scratch.add_(grad.float()) if add else scratch.copy_(grad.float())
+        partial.zero_()
+        partial[0] = scratch.double().square().sum()
+        grad.zero_()
+        self.launches += 1
+        self.log.append((kind, grad.numel()))
+
+    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
+        self._stage1("norm", grad, scratch, partial, add=False)
+
+    def fused_accum_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
+        self._stage1("accum", grad, scratch, partial, add=True)
+
+    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
+        total = torch.tensor(math.sqrt(float(partials.sum())) * grad_scale, dtype=torch.float32)
+        clip[1] = total
+        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
+        self.launches += 1
+        self.log.append(("coef", None))
+
+    def barrier(self, channel=2, stream=None):
+        self.log.append(("barrier", None))
+
+    def lars_segments(self, table, shard_vecs, ntensors):
+        self.nslots_of = getattr(self, "nslots_of", {})
+        t = torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
+        self.nslots_of[id(t)] = check_lars_segments(table, shard_vecs, ntensors)
+        return t
+
+    def lars_tensors(self, table, nslots):
+        check_lars_tensors(table, nslots)
+        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
+
+    def fused_lars_norm(self, master, scratch, segs, slots, dtype, nblocks=0, stream=None):
+        e = 16 // torch.empty((), dtype=dtype).element_size()
+        assert slots.shape == (self.nslots_of[id(segs)], 2)
+        for vec0, nvec, _, slot0 in segs.tolist():
+            for c in range((nvec + LARS_CHUNK - 1) // LARS_CHUNK):
+                a, b = (vec0 + c * LARS_CHUNK) * e, (vec0 + min(nvec, (c + 1) * LARS_CHUNK)) * e
+                slots[slot0 + c] = torch.stack([master[a:b].double().square().sum(), scratch[a:b].double().square().sum()])
+        self.launches += 1
+        self.log.append(("lars_norm", master.numel()))
+
+    def fused_lars_trust(self, slots, tensors, xchg, clip, hp, scal, trust, channel=0, stream=None):
+        assert xchg.numel() >= 2 * self.world * tensors.shape[0]
+        f = lambda v: torch.tensor(float(v), dtype=torch.float32)  # noqa: E731
+        gscale, wd, eta, eps, coef = f(hp[3]), f(hp[2]), f(hp[4]), f(hp[5]), f(clip[2])
+        for j, (slot0, n, excluded, _) in enumerate(tensors.tolist()):
+            w2, g2 = (float(v) for v in slots[slot0:slot0 + n].sum(0)) if n else (0.0, 0.0)
+            wn, gn = f(math.sqrt(w2)), f(math.sqrt(g2) * float(gscale) * float(coef))
+            t = torch.tensor(1.0)
+            if not excluded and wn != 0 and gn != 0:
+                t = eta * wn / (gn + wd * wn + eps)
+            scal[j, 0] = gscale * coef * t
+            scal[j, 1] = wd * t if not excluded and wn != 0 and gn != 0 else 0.0
+            trust[j] = t
+        self.launches += 1
+        self.log.append(("lars_trust", tensors.shape[0]))
+
+    def fused_lars_apply(self, param, scratch, segs, scal, hp, master, mom, channel=0, nblocks=0, stream=None):
+        lr, mu = float(hp[0]), float(hp[1])
+        e = 16 // param.element_size()
+        for vec0, nvec, tensor, _ in segs.tolist():
+            s = slice(vec0 * e, (vec0 + nvec) * e)
+            d = scratch[s] * scal[tensor, 0] + scal[tensor, 1] * master[s]
+            mom[s].mul_(mu).add_(d)
+            master[s].sub_(lr * mom[s])
+        param.copy_(master.to(param.dtype))
+        self.launches += 1
+        self.log.append(("lars_apply", param.numel()))
+
+
+# ------------------------------------------------------------------ the segment tables
+def _tables(numels, es, world, bucket_mb):
+    plan, _ = plan_buckets(numels, es, world, bucket_mb)
+    return plan, {(k, r): lars_segments(m, numels, s, n, es, world, r) for k, (s, n, m) in enumerate(plan) for r in range(world)}
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 8])
+@pytest.mark.parametrize("es", [2, 4])
+def test_segment_tables_cover_every_shard_and_every_element_once(world, es):
+    # odd sizes: a 1-element bias, tensors of one vector and less, one tensor wider than a shard, 2 chunks and a tail
+    numels = [1, 7, 8, 9, 64 * 3 * 3 * 3, 5, 1000, 2 * LARS_CHUNK * 8 + 3, 17, 4096, 3]
+    per_vec = 16 // es
+    plan, tables = _tables(numels, es, world, 0.05)
+    assert len(plan) >= 2
+    for k, (start, numel, members) in enumerate(plan):
+        shard = numel // world // per_vec
+        owner = {}                                   # element of the flat buffer -> tensor of the segment holding it
+        for r in range(world):
+            t = tables[(k, r)]
+            nslots = check_lars_segments(t, shard, len(numels))
+            assert nslots == sum((n + LARS_CHUNK - 1) // LARS_CHUNK for _, n, _, _ in t)
+            assert len({pi for _, _, pi, _ in t}) == len(t), "a tensor with two segments on one rank"
+            for vec0, nvec, pi, _ in t:
+                lo = start + (r * shard + vec0) * per_vec
+                for x in range(lo, lo + nvec * per_vec):
+                    assert x not in owner
+                    owner[x] = pi
+        assert sorted(owner) == list(range(start, start + numel))            # every element exactly once
+        for pi, off in members:                                              # ... and a tensor's own in its segments
+            assert all(owner[x] == pi for x in range(off, off + numels[pi]))
+    if world > 1:                                                            # some tensor straddles a shard boundary
+        straddle = [pi for (k, r), t in tables.items() for _, _, pi, _ in t
+                    if any(pi == q for rr in range(world) if rr != r for _, _, q, _ in tables[(k, rr)])]
+        assert straddle
+
+
+def test_padding_only_shard_and_rejected_tables():
+    # world 8, bf16: a bucket of 64 * 8 elements holding 9 -> shards 2..7 are padding only, owned by the last tensor
+    t = [lars_segments([(0, 0)], [9], 0, 64 * 8, 2, 8, r) for r in range(8)]
+    assert t[0] == [[0, 8, 0, 0]] and t[1] == [[0, 8, 0, 0]] and t[7] == [[0, 8, 0, 0]]
+    good = [[0, 3, 0, 0], [3, LARS_CHUNK + 1, 1, 1], [LARS_CHUNK + 4, 4, 2, 3]]
+    assert check_lars_segments(good, LARS_CHUNK + 8, 3) == 4
+    bad = [
+        [],                                                        # empty
+        [[0, 3, 0, 0], [3, LARS_CHUNK + 1, 1, 1]],                 # does not reach the shard's end
+        [[1, 2, 0, 0], [3, LARS_CHUNK + 5, 1, 1]],                 # does not start at 0
+        [[0, 3, 0, 0], [2, LARS_CHUNK + 6, 1, 1]],                 # overlap
+        [[0, 3, 0, 0], [4, LARS_CHUNK + 4, 1, 1]],                 # gap
+        [[0, 3, 0, 0], [3, 0, 1, 1], [3, LARS_CHUNK + 5, 2, 1]],   # empty segment
+        [[0, 3, 0, 0], [3, LARS_CHUNK + 5, 3, 1]],                 # tensor out of range
+        [[0, 3, -1, 0], [3, LARS_CHUNK + 5, 1, 1]],                # negative tensor
+        [[0, 3, 0, 0], [3, LARS_CHUNK + 5, 1, 2]],                 # wrong slot0
+        [[0, LARS_CHUNK + 16, 0, 0]],                              # past the shard
+    ]
+    for b in bad:
+        with pytest.raises(ValueError):
+            check_lars_segments(b, LARS_CHUNK + 8, 3)
+    check_lars_tensors([[0, 2, 0, 0], [2, 0, 1, 0]], 2)
+    for b in ([[0, 3, 0, 0]], [[-1, 1, 0, 0]], [[1, -1, 0, 0]], []):
+        with pytest.raises(ValueError):
+            check_lars_tensors(b, 2)
+
+
+# ------------------------------------------------------------------ the engine against float64 LARC + SGD
+LARS = dict(lr=0.5, momentum=0.9, weight_decay=5e-4, trust_coefficient=0.02, eps=1e-8)
+BATCH = 8
+
+
+def _batch(step, channels_last=True):
+    torch.manual_seed(200 + step)
+    x, y = torch.randn(BATCH, 3, 8, 8), torch.randint(0, 10, (BATCH,))
+    return (x.contiguous(memory_format=torch.channels_last) if channels_last else x), y
+
+
+def larc_step(params, opt, wd, eta, eps):
+    """NVIDIA Apex LARC(clip=False) on the .grad of `params` (float64), then `opt` (torch.optim.SGD, weight_decay=0)."""
+    with torch.no_grad():
+        for p in params:
+            if p.grad is None or p.dim() <= 1:
+                continue
+            wn, gn = p.norm(), p.grad.norm()
+            if wn != 0 and gn != 0:
+                t = eta * wn / (gn + wn * wd + eps)
+                p.grad.add_(p, alpha=wd).mul_(t)
+    opt.step()
+
+
+def _pair(channels_last=True, model=None, **kw):
+    make = model or _model
+    ref, net = make(channels_last).double(), make(channels_last)
+    opt = torch.optim.SGD(ref.parameters(), lr=LARS["lr"], momentum=LARS["momentum"])
+    eng = BnetDDP(net, optimizer="lars", bucket_mb=0.002, comm=LarsComm(), **LARS, **kw)
+    return ref, opt, net, eng
+
+
+def _ref_step(ref, opt, x, y, k, max_norm, lr):
+    for g in opt.param_groups:
+        g["lr"] = lr
+    opt.zero_grad()
+    for xs, ys in zip(x.split(BATCH // k), y.split(BATCH // k)):
+        (torch.nn.functional.cross_entropy(ref(xs.double()), ys) / k).backward()
+    norm = torch.nn.utils.clip_grad_norm_(ref.parameters(), max_norm if max_norm is not None else math.inf)
+    larc_step(list(ref.parameters()), opt, LARS["weight_decay"], LARS["trust_coefficient"], LARS["eps"])
+    return float(norm)
+
+
+@pytest.mark.parametrize("k", [1, 2])
+@pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
+@pytest.mark.parametrize("direct_grads", ["1", "0"], ids=["adopted", "accumulated"])
+@pytest.mark.parametrize("channels_last", [True, False])
+def test_lars_engine_trains_like_larc_and_sgd(cpu_engine, k, clipped, direct_grads, channels_last):
+    cpu_engine.setenv("BNET_DIRECT_GRADS", direct_grads)
+    thr = 0.05 if clipped else None
+    ref, opt, net, eng = _pair(channels_last, max_grad_norm=thr, accumulation_steps=k)
+    assert len(eng.buckets) >= 2 and eng._staged
+    lr = LARS["lr"]
+    for step in range(4):
+        if step == 2:
+            lr = 0.2
+            eng.set_lr(lr)                                          # mid-run: the device block, no re-capture
+        x, y = _batch(step, channels_last)
+        want = _ref_step(ref, opt, x, y, k, thr, lr)
+        eng.train_step(x, y)
+        if clipped:
+            assert float(eng.last_grad_norm) == pytest.approx(want, rel=1e-5)
+        assert float(eng.flat_grad.abs().max()) == 0.0
+        for a, b in zip(net.parameters(), ref.parameters()):
+            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5), (step, float((a.double() - b).abs().max()))
+        t = eng.last_trust_ratios
+        assert t.shape == (len(list(net.parameters())),) and t.dtype == torch.float32
+        for ti, p in zip(t.tolist(), net.parameters()):
+            assert (ti == 1.0) if p.dim() <= 1 else (0.0 < ti < math.inf and ti != 1.0)
+    assert float(eng._hp[0]) == pytest.approx(0.2) and float(eng._hp[4]) == pytest.approx(LARS["trust_coefficient"])
+
+
+@pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
+@pytest.mark.parametrize("k", [1, 2])
+def test_launch_order(cpu_engine, clipped, k):
+    ref, opt, net, eng = _pair(max_grad_norm=1.0 if clipped else None, accumulation_steps=k)
+    nb, comm = len(eng.buckets), eng.comm
+    for step in range(2):
+        n0, l0 = len(comm.log), comm.launches
+        eng.train_step(*_batch(step))
+        kinds = [kind for kind, _ in comm.log[n0:]]
+        want = ["norm"] * nb + ["accum"] * nb * (k - 1) + (["coef"] if clipped else [])
+        want += ["lars_norm"] * nb + ["lars_trust"] + ["lars_apply"] * nb
+        assert kinds == want                                        # (no bare barrier: the trust kernel's stands for it)
+        assert comm.launches - l0 == len(want)
+        assert [n for kind, n in comm.log[n0:] if kind == "lars_apply"] == [b.numel for b in eng.buckets]
+
+
+def test_other_optimizers_have_no_trust_ratios(cpu_engine):
+    for kw in ({}, {"optimizer": "adamw"}):
+        eng = BnetDDP(_model(), bucket_mb=0.002, comm=LarsComm(), **kw)
+        assert eng.last_trust_ratios is None
+
+
+class _Branchy(torch.nn.Module):
+    def __init__(self, channels_last=True):
+        super().__init__()
+        torch.manual_seed(4)
+        self.unused = torch.nn.Linear(32, 32, bias=False)
+        self.net = _model(channels_last)
+
+    def forward(self, x):
+        return self.net(x)
+
+
+def test_bucket_without_gradient_is_left_alone(cpu_engine):
+    ref, opt, net, eng = _pair(model=_Branchy)
+    idle = [k for k, b in enumerate(eng.buckets) if len(b.params) == 1 and b.params[0] is net.unused.weight]
+    assert len(idle) == 1
+    w0 = net.unused.weight.detach().clone()
+    eng._lars_slots.fill_(7.0)                                       # stale sums must not reach the ratios
+    for step in range(2):
+        x, y = _batch(step)
+        ref.unused.weight.grad = None
+        _ref_step(ref, opt, x, y, 1, None, LARS["lr"])
+        eng.train_step(x, y)
+        for a, b in zip(net.parameters(), ref.parameters()):
+            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5)
+    assert torch.equal(net.unused.weight, w0)
+    assert float(eng.last_trust_ratios[0]) == 1.0                    # (`unused` is the first parameter)
+    assert [kind for kind, _ in eng.comm.log].count("lars_apply") == 2 * (len(eng.buckets) - 1)
+
+
+def test_state_dict_round_trip_and_keys(cpu_engine):
+    ref, opt, net, eng = _pair()
+    eng.train_step(*_batch(0))
+    state = eng.optimizer_state_dict()
+    assert set(state) == {"optimizer", "lr", "momentum", "weight_decay", "trust_coefficient", "eps", "world", "rank", "buckets"}
+    assert state["optimizer"] == "lars" and all(set(b) == {"master", "momentum"} for b in state["buckets"])
+    resumed = _pair()[3]
+    resumed.load_optimizer_state_dict(copy.deepcopy(state))
+    for b1, b2 in zip(resumed.buckets, eng.buckets):
+        assert all(torch.equal(t1, t2) for t1, t2 in zip(b1.state, b2.state))
+    assert torch.equal(resumed._hp, eng._hp)
+    for other in ({}, {"optimizer": "adamw"}):
+        plain = BnetDDP(_model(), bucket_mb=0.002, comm=LarsComm(), **other)
+        with pytest.raises(ValueError):
+            plain.load_optimizer_state_dict(copy.deepcopy(state))
+        with pytest.raises(ValueError):
+            resumed.load_optimizer_state_dict(copy.deepcopy(plain.optimizer_state_dict()))
+
+
+def test_rejects_bad_arguments(cpu_engine):
+    for bad in ({"trust_coefficient": 0.0}, {"trust_coefficient": -1e-3}, {"trust_coefficient": float("nan")},
+                {"eps": -1e-8}, {"eps": float("nan")}, {"amsgrad": True}, {"maximize": True}):
+        with pytest.raises(ValueError):
+            BnetDDP(_model(), optimizer="lars", bucket_mb=0.002, comm=LarsComm(), **bad)
+    with pytest.raises(ValueError):
+        BnetDDP(_model(), optimizer="lamb", bucket_mb=0.002, comm=LarsComm())
