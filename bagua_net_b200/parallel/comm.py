@@ -124,6 +124,8 @@ def _declare(lib):
     lib.bnet_fused_lars_norm.argtypes = [vp, sz, i, vp, vp, vp, i, vp, i, i, vp]
     lib.bnet_fused_lars_trust.argtypes = [vp, vp, vp, i, sz, vp, vp, vp, vp, i, vp]
     lib.bnet_fused_lars_apply.argtypes = [vp, sz, sz, i, vp, vp, i, vp, vp, vp, vp, i, i, vp]
+    lib.bnet_ema_update.argtypes = [vp, sz, vp, vp, vp, i, vp]
+    lib.bnet_ema_advance.argtypes = [vp, vp, vp]
     lib.bnet_pack_cast.argtypes = [vp, i, vp, i, i, C.c_float, C.c_uint64, vp]
 
 
@@ -461,6 +463,26 @@ class SymmComm:
             self.h, self.offset_of(param), param.numel(), DT[param.dtype], C.c_void_p(scratch.data_ptr()),
             C.c_void_p(segs.data_ptr()), segs.shape[0], C.c_void_p(scal.data_ptr()), C.c_void_p(hp.data_ptr()),
             C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), channel, nblocks, self._stream(stream)), "fused_lars_apply")
+        self.launches += n
+
+    # ------------------------------------------------------------------ exponential moving average of the master weights
+    def ema_update(self, master: torch.Tensor, ema: torch.Tensor, blk: torch.Tensor, nblocks: int = 0, stream=None):
+        """Per bucket, after the optimizer step's last update: on an EMA step of the 4-float device block ``blk``
+        ({1 - decay, every, step, n_averaged}), ``ema`` becomes a copy of ``master`` (n_averaged == 0) or
+        ``torch.lerp(ema, master, 1 - decay)``; on other steps neither is touched.  Both are this rank's fp32 shards."""
+        assert master.is_cuda and master.dtype == torch.float32 and master.is_contiguous()
+        assert ema.is_cuda and ema.dtype == torch.float32 and ema.is_contiguous() and ema.numel() == master.numel()
+        assert blk.is_cuda and blk.dtype == torch.float32 and blk.numel() >= 4 and blk.is_contiguous()
+        n = self._chk(self.lib.bnet_ema_update(self.h, master.numel(), C.c_void_p(master.data_ptr()),
+                                               C.c_void_p(ema.data_ptr()), C.c_void_p(blk.data_ptr()), nblocks,
+                                               self._stream(stream)), "ema_update")
+        self.launches += n
+
+    def ema_advance(self, blk: torch.Tensor, stream=None):
+        """Once per optimizer step, after every bucket's ``ema_update``: count the step in ``blk``, and the EMA update
+        when it was an EMA step."""
+        assert blk.is_cuda and blk.dtype == torch.float32 and blk.numel() >= 4 and blk.is_contiguous()
+        n = self._chk(self.lib.bnet_ema_advance(self.h, C.c_void_p(blk.data_ptr()), self._stream(stream)), "ema_advance")
         self.launches += n
 
     # ------------------------------------------------------------------ collectives on ordinary tensors

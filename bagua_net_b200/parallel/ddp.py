@@ -15,6 +15,8 @@ NVSwitch box:
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 import torch.distributed as dist
 
@@ -174,8 +176,18 @@ def _check_max_norm(v) -> float:
     return v
 
 
+def _check_ema_decay(v) -> float:
+    try:
+        v = float(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"ema_decay must be a number in [0, 1] (got {v!r})") from None
+    if not 0.0 <= v <= 1.0:               # (False for NaN as well)
+        raise ValueError(f"ema_decay must be in [0, 1] (got {v})")
+    return v
+
+
 class _Bucket:
-    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state", "scratch", "partial", "launched")
+    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state", "scratch", "partial", "launched", "ema")
 
     def __init__(self):
         self.params = []
@@ -185,6 +197,7 @@ class _Bucket:
         self.scratch = None          # staged step: this rank's fp32 shard of the rank-summed (accumulated) gradient
         self.partial = None          # staged step: the bucket's row of per-CTA sums of squares
         self.launched = False        # staged step: stage 1 ran for this bucket in the current step (the scratch holds data)
+        self.ema = None              # EMA of the master shard (fp32, same layout), kept apart from the optimizer's state
 
     @property
     def master(self) -> torch.Tensor:
@@ -218,14 +231,29 @@ class BnetDDP(torch.nn.Module):
     ``loss.backward(); engine.finish_step()`` once per micro-batch with the UNSCALED micro-batch loss (the mean over the
     micro-batch) -- do not divide it by k, the engine does that.  ``micro_step`` tells where in the step you are.
     BatchNorm statistics are per micro-batch, as with accumulation in torch.  ``1`` keeps the single-batch step.
+
+    ema_decay: keep an exponential moving average of the fp32 master weights, as
+    ``torch.optim.swa_utils.AveragedModel(module, multi_avg_fn=get_ema_multi_avg_fn(ema_decay), use_buffers=False)``
+    with ``update_parameters`` called after every ``ema_every``-th optimizer step (steps counted from 1): the first
+    update copies the masters, later ones take ``torch.lerp(ema, master, 1 - ema_decay)``.  Each rank keeps the EMA of
+    its own master shards, and the update runs on the device behind the step's last update, so a captured CUDA graph
+    decides on its own which steps update.  Buffers (BatchNorm statistics) are not averaged.  Evaluate or save the
+    averaged model inside ``with engine.ema_parameters():``; ``set_ema_decay`` and ``reset_ema`` change it between steps.
+    ``None`` keeps no EMA.
     """
 
     def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float | None = None, weight_decay: float = 0.0,
                  bucket_mb: float = 64.0, comm: SymmComm | None = None, extra_heap_bytes: int = 64 << 20,
                  nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None,
-                 accumulation_steps: int = 1, trust_coefficient: float = 0.001):
+                 accumulation_steps: int = 1, trust_coefficient: float = 0.001, ema_decay: float | None = None,
+                 ema_every: int = 1):
         super().__init__()
+        if ema_decay is not None:
+            ema_decay = _check_ema_decay(ema_decay)
+        if isinstance(ema_every, bool) or not isinstance(ema_every, int) or not 1 <= ema_every <= 1 << 24:
+            # (the device block counts in floats, exact up to 2^24)
+            raise ValueError(f"ema_every must be an int in [1, 2^24] (got {ema_every!r})")
         if isinstance(accumulation_steps, bool) or not isinstance(accumulation_steps, int) or accumulation_steps < 1:
             raise ValueError(f"accumulation_steps must be an int >= 1 (got {accumulation_steps!r})")
         if max_grad_norm is not None:
@@ -344,6 +372,8 @@ class BnetDDP(torch.nn.Module):
             b.param = self.flat_param[b.start:b.start + b.numel]
             shard = b.numel // comm.world
             master = b.param[comm.rank * shard:(comm.rank + 1) * shard].float().contiguous()
+            if ema_decay is not None and dtype == torch.float32:
+                master = master.clone()   # (else a view of the parameters, which ema_parameters() overwrites)
             b.state = (master,) + tuple(torch.zeros_like(master) for _ in _STATE_NAMES[optimizer][1:])
         # AdamW and LARS always read their hyper-parameters (and AdamW its step count) from device memory
         # (csrc/cuda/optim_body.cuh); SGD passes them as launch arguments until the first set_lr
@@ -373,6 +403,12 @@ class BnetDDP(torch.nn.Module):
         self.max_grad_norm = max_grad_norm
         if optimizer == "lars":
             self._lars_setup(params, plan, es, dev)
+        # the EMA of the master shards, starting as their copy (AveragedModel deep-copies the model), and its device block
+        self.ema_decay, self.ema_every, self._ema, self._in_ema = ema_decay, ema_every, None, False
+        if ema_decay is not None:
+            for b in self.buckets:
+                b.ema = b.master.clone()
+            self._ema = torch.tensor(self._ema_block(0, 0), dtype=torch.float32, device=dev)
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1)
         self.grad_copies = 0             # gradients that had to be copied into their slice (not written there by their producer)
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad) for p in params]
@@ -420,6 +456,7 @@ class BnetDDP(torch.nn.Module):
         """Make the updated parameters visible to the compute stream (call after backward).  With
         ``accumulation_steps=k``, call it after every micro-batch's backward: the first k-1 calls only reduce that
         micro-batch's gradients into the scratch, the k-th also updates."""
+        self._check_not_in_ema("finish_step")
         for b in self.buckets:
             if b.ready:                           # parameters that got no gradient this step
                 self._launch(b)
@@ -434,6 +471,12 @@ class BnetDDP(torch.nn.Module):
         if self._inflight:
             if self._staged:
                 self._staged_update()
+            if self._ema is not None:
+                # behind the step's last update, on the comm stream: every bucket's EMA shard (the kernels skip the
+                # steps that are not EMA steps on the device), then the step count
+                for b in self.buckets:
+                    self.comm.ema_update(b.master, b.ema, self._ema, nblocks=self.nblocks, stream=self.comm_stream)
+                self.comm.ema_advance(self._ema, stream=self.comm_stream)
             if self.optimizer == "adamw":
                 # one optimizer step taken: advance the step count the kernels read, behind this step's last bucket
                 # (on the comm stream, so a captured step replays it)
@@ -574,12 +617,13 @@ class BnetDDP(torch.nn.Module):
         with torch.cuda.stream(side):               # warm-up on a side stream (cuDNN autotune, allocator)
             # The warm-up runs REAL steps (the fused optimizer included: every rank has to take part in its
             # barriers), so everything a step mutates is saved first and put back afterwards — parameters, fp32
-            # optimizer state, the hyper-parameter block (AdamW's step count), module buffers (BatchNorm running
-            # statistics).  A (re)capture therefore leaves the training trajectory exactly where eager mode would
-            # have it; checkpoint/resume stays step-exact.
+            # optimizer state, the hyper-parameter block (AdamW's step count), the EMA shards and block, module buffers
+            # (BatchNorm running statistics).  A (re)capture therefore leaves the training trajectory exactly where
+            # eager mode would have it; checkpoint/resume stays step-exact.
             live = [self.flat_param] + [t for b in self.buckets for t in b.state]
+            live += [b.ema for b in self.buckets if b.ema is not None]
             live += [t for t in self.module.buffers() if t.is_cuda and t.numel()]
-            live += [t for t in (self._hp, self._clip) if t is not None]
+            live += [t for t in (self._hp, self._clip, self._ema) if t is not None]
             saved = [t.clone() for t in live]
             for _ in range(2):
                 self._eager_step(self._gx, self._gy, loss_fn)
@@ -611,6 +655,7 @@ class BnetDDP(torch.nn.Module):
         ``accumulation_steps=k``: k micro-batches of ``inputs.shape[0] // k`` samples and one update; the loss returned
         is the mean of the k micro-batch losses."""
         k = self.accumulation_steps
+        self._check_not_in_ema("train_step")
         if self._micro:
             raise ValueError(f"train_step called in the middle of an accumulation step (micro_step={self._micro}): "
                              "finish that step with backward + finish_step first")
@@ -732,8 +777,13 @@ class BnetDDP(torch.nn.Module):
         else:
             head = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
         names = _STATE_NAMES[self.optimizer]
-        return {**head, "world": self.comm.world, "rank": self.comm.rank,
-                "buckets": [{k: t.detach().cpu() for k, t in zip(names, b.state)} for b in self.buckets]}
+        buckets = [{k: t.detach().cpu() for k, t in zip(names, b.state)} for b in self.buckets]
+        if self._ema is not None:
+            step, n_averaged = (int(v) for v in self._ema[self._EMA_STEP:].tolist())
+            head.update(ema_decay=self.ema_decay, ema_every=self.ema_every, ema_step=step, ema_n_averaged=n_averaged)
+            for d, b in zip(buckets, self.buckets):
+                d["ema"] = b.ema.detach().cpu()
+        return {**head, "world": self.comm.world, "rank": self.comm.rank, "buckets": buckets}
 
     def load_optimizer_state_dict(self, state: dict) -> None:
         self._check_step_boundary("load an optimizer state")
@@ -742,11 +792,24 @@ class BnetDDP(torch.nn.Module):
             raise ValueError(f"optimizer state of {kind!r} cannot be loaded into a {self.optimizer!r} engine")
         if state["world"] != self.comm.world or state["rank"] != self.comm.rank or len(state["buckets"]) != len(self.buckets):
             raise ValueError("optimizer state was saved for a different world size / rank / bucket layout")
+        has_ema = "ema_decay" in state
+        if has_ema and self._ema is None:
+            raise ValueError("the optimizer state holds an EMA of the weights, which this engine would drop: build it with "
+                             "ema_decay=... to load it")
         for b, s in zip(self.buckets, state["buckets"]):
-            if s["master"].shape != b.master.shape:
+            if s["master"].shape != b.master.shape or (has_ema and s["ema"].shape != b.master.shape):
                 raise ValueError("optimizer state shard does not match this bucket")
+        for b, s in zip(self.buckets, state["buckets"]):
             for k, t in zip(_STATE_NAMES[self.optimizer], b.state):
                 t.copy_(s[k])
+        if self._ema is not None:
+            # a state without an EMA (fine-tuning from a plain checkpoint): the EMA restarts from the loaded masters
+            if has_ema:
+                self.ema_decay, self.ema_every = _check_ema_decay(state["ema_decay"]), int(state["ema_every"])
+            for b, s in zip(self.buckets, state["buckets"]):
+                b.ema.copy_(s["ema"] if has_ema else b.master)
+            counts = (state["ema_step"], state["ema_n_averaged"]) if has_ema else (0, 0)
+            self._ema.copy_(torch.tensor(self._ema_block(*counts), dtype=torch.float32))
         if self.optimizer == "adamw":
             self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
             self.betas = tuple(state["betas"])
@@ -764,7 +827,8 @@ class BnetDDP(torch.nn.Module):
             self._graph = None                # hyper-parameters are baked into a captured step
 
     def sync_master_from_params(self) -> None:
-        """After module.load_state_dict(): rebuild the fp32 master shards from the (just loaded) parameters."""
+        """After module.load_state_dict(): rebuild the fp32 master shards from the (just loaded) parameters.  The EMA
+        of the weights is left as it is; call ``reset_ema()`` as well to restart it from the loaded weights."""
         for b in self.buckets:
             shard = b.numel // self.comm.world
             b.master.copy_(b.param[self.comm.rank * shard:(self.comm.rank + 1) * shard].float())
@@ -826,6 +890,75 @@ class BnetDDP(torch.nn.Module):
 
     # AdamW's hyper-parameter block: {lr, beta1, beta2, eps, weight_decay, grad_scale, step, reserved}
     _HP_STEP = 6
+
+    # ------------------------------------------------------------------ exponential moving average of the weights
+    # The EMA block (csrc/cuda/optim_body.cuh): {1 - decay, every, step, n_averaged}
+    _EMA_STEP = 2
+
+    def _ema_block(self, step: int, n_averaged: int) -> list:
+        # 1 - decay in double, rounded once to fp32: the weight torch._foreach_lerp_ gets from get_ema_multi_avg_fn
+        return [1.0 - self.ema_decay, float(self.ema_every), float(step), float(n_averaged)]
+
+    def _require_ema(self, what: str) -> None:
+        if self._ema is None:
+            raise ValueError(f"cannot {what}: the engine keeps no EMA of the weights (build it with ema_decay=...)")
+
+    def _check_not_in_ema(self, what: str) -> None:
+        if self._in_ema:
+            raise ValueError(f"{what} inside ema_parameters(): the parameters hold the EMA weights, not the trained ones")
+
+    def set_ema_decay(self, decay: float) -> None:
+        """Change the EMA's decay (a warm-up schedule, say).  The update kernels read it from device memory, so a
+        captured CUDA graph follows it without being re-captured."""
+        self._require_ema("set the EMA decay")
+        self.ema_decay = _check_ema_decay(decay)
+        self._ema[:1].copy_(torch.tensor([1.0 - self.ema_decay], dtype=torch.float32))
+
+    def reset_ema(self) -> None:
+        """Set the EMA's update count to 0 on the device, so that its next update copies the master weights (what
+        ``model_ema.n_averaged.fill_(0)`` does for an ``AveragedModel``).  The step count goes on."""
+        self._require_ema("reset the EMA")
+        self._ema[self._EMA_STEP + 1:].zero_()
+
+    @contextlib.contextmanager
+    def ema_parameters(self):
+        """Inside the block the module's parameters are the EMA weights, rounded to the parameter dtype, on every rank:
+        for evaluation, or for ``module.state_dict()`` of the averaged model.  On exit they are the trained parameters
+        again, bitwise.  Collective: every rank enters and leaves together.  ``train_step`` and ``finish_step`` raise
+        inside it.  Yields the module."""
+        self._require_ema("swap in the EMA weights")
+        self._check_step_boundary("swap in the EMA weights")
+        if self._in_ema:
+            raise ValueError("ema_parameters() is already active")
+        if self.flat_param.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise ValueError("ema_parameters() cannot run inside a CUDA graph capture")
+        self._publish(lambda b: b.ema)
+        self._in_ema = True
+        try:
+            yield self.module
+        finally:
+            self._in_ema = False
+            self._publish(lambda b: b.master)
+
+    def _publish(self, shard_of) -> None:
+        """Every rank writes ``shard_of(bucket)`` (an fp32 shard laid out as the master), rounded to the parameter dtype
+        as the update kernels round, into its part of every rank's parameters, on the current stream.  The opening
+        barrier means every rank is done with its step and with reading the parameters; the closing one, that every
+        rank's parameters are complete."""
+        cur = torch.cuda.current_stream()
+        cur.wait_stream(self.comm_stream)
+        world, rank = self.comm.world, self.comm.rank
+        if world > 1:
+            self.comm.barrier(stream=cur)
+        with torch.no_grad():
+            for b in self.buckets:
+                shard = b.numel // world
+                src = shard_of(b).to(self.dtype)
+                mine = b.param[rank * shard:(rank + 1) * shard]
+                for peer in range(world):
+                    (mine if peer == rank else self.comm.peer_tensor(mine, peer)).copy_(src)
+        if world > 1:
+            self.comm.barrier(stream=cur)
 
     def _adamw_hp(self, step: int) -> list:
         return [self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, self._grad_scale, float(step), 0.0]

@@ -939,6 +939,59 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_lars_apply_kernel(CollDev d,
                        state, 0, chan);
 }
 
+// ------------------------------------------------------------------ exponential moving average of the master weights
+// One batch of the EMA update: U float4s of the master shard (and of the EMA shard unless COPY) per thread, every load
+// issued before any math, non-temporal as in fused_batch.
+template <int U, bool COPY>
+__device__ __forceinline__ void ema_batch(const float4* __restrict__ master, float4* __restrict__ ema, size_t i, size_t stride,
+                                          float w) {
+  float4 m[U], e[COPY ? 1 : U];
+#pragma unroll
+  for (int u = 0; u < U; u++) m[u] = ptx::ld_na_f4(master + i + u * stride);
+  if constexpr (!COPY) {
+#pragma unroll
+    for (int u = 0; u < U; u++) e[u] = ptx::ld_na_f4(ema + i + u * stride);
+  }
+#pragma unroll
+  for (int u = 0; u < U; u++) {
+    float4 r = m[u];
+    if constexpr (!COPY) {
+      r.x = optim::ema_lerp(e[u].x, m[u].x, w); r.y = optim::ema_lerp(e[u].y, m[u].y, w);
+      r.z = optim::ema_lerp(e[u].z, m[u].z, w); r.w = optim::ema_lerp(e[u].w, m[u].w, w);
+    }
+    ptx::st_na_f4(ema + i + u * stride, r);
+  }
+}
+
+template <bool COPY>
+__device__ __forceinline__ void ema_body(const float4* __restrict__ master, float4* __restrict__ ema, size_t n4, float w) {
+  constexpr int U = 4;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+  for (; i + (U - 1) * stride < n4; i += U * stride) ema_batch<U, COPY>(master, ema, i, stride, w);
+  for (; i < n4; i += stride) ema_batch<1, COPY>(master, ema, i, stride, w);
+}
+
+// Per bucket, after the optimizer step's last update launch: on an EMA step (optim::ema_gate on the block), this rank's
+// fp32 EMA shard becomes a copy of the master shard (no update averaged yet) or lerp(ema, master, weight).  On any other
+// step every thread exits after reading the block, before touching either shard.  Rank-local, no barriers, no atomics:
+// each element's bits depend on neither the grid nor a repeat.
+__global__ void __launch_bounds__(kThreads) bnet_ema_update_kernel(const float4* __restrict__ master, float4* __restrict__ ema,
+                                                                  size_t n4, const float* __restrict__ blk) {
+  const optim::EmaGate g = optim::ema_gate(blk[optim::kEmaStep], blk[optim::kEmaEvery], blk[optim::kEmaNAveraged]);
+  if (!g.update) return;
+  if (g.copy) ema_body<true>(master, ema, n4, 0.0f);
+  else ema_body<false>(master, ema, n4, blk[optim::kEmaWeight]);
+}
+
+// Once per optimizer step, one thread, after every bucket's bnet_ema_update_kernel: count the step, and the update when
+// it was an EMA step.  A kernel, not a host-side add, because the second increment depends on device values.
+__global__ void bnet_ema_advance_kernel(float* __restrict__ blk) {
+  const optim::EmaGate g = optim::ema_gate(blk[optim::kEmaStep], blk[optim::kEmaEvery], blk[optim::kEmaNAveraged]);
+  if (g.update) blk[optim::kEmaNAveraged] += 1.0f;
+  blk[optim::kEmaStep] += 1.0f;
+}
+
 // ------------------------------------------------------------------ multi-tensor pack + cast (K5)
 template <typename S, typename D>
 __global__ void __launch_bounds__(256) bnet_pack_cast_kernel(const BnetPackItem* __restrict__ items, D* __restrict__ dst,
@@ -1671,6 +1724,34 @@ BNET_API int bnet_fused_lars_apply(BnetColl* c, size_t param_off, size_t count, 
     return -1;
   return run_fused_kernel<LarsApplyKernel>(c, dtype, f, f.poff, f.nvec, scratch, reinterpret_cast<const int4*>(segs), nseg,
                                            reinterpret_cast<const float2*>(scal), hp, master, mom_buf, channel);
+}
+
+// ---- exponential moving average of the master weights
+static int ema_block_check(const float* blk) {
+  if (!blk || ((uintptr_t)blk & 15)) return fail("EMA block must be a 16-byte aligned device pointer");
+  return 0;
+}
+
+BNET_API int bnet_ema_update(BnetColl* c, size_t count, const float* master, float* ema, const float* blk, int nblocks, void* stream) {
+  if (count == 0 || count % 4) return fail("EMA update needs a whole number (>= 1) of float4s");
+  if (((uintptr_t)master | (uintptr_t)ema) & 15) return fail("EMA shards must be 16-byte aligned");
+  if (ema_block_check(blk) < 0) return -1;
+  const size_t n4 = count / 4;
+  int nb = nblocks;
+  if (nb <= 0) {   // two CTAs per SM, no more than give every thread one batch of 4 vectors
+    nb = (int)env_int("COLL_BLOCKS_SINGLE", 264);
+    const size_t want = (n4 + kThreads * 4 - 1) / (kThreads * 4);
+    if ((size_t)nb > want) nb = (int)want;
+  }
+  if (nb > BNET_COLL_MAX_BLOCKS) nb = BNET_COLL_MAX_BLOCKS;
+  if (nb < 1) nb = 1;
+  return launch(bnet_ema_update_kernel, nb, kThreads, (cudaStream_t)stream, reinterpret_cast<const float4*>(master),
+                reinterpret_cast<float4*>(ema), n4, blk);
+}
+
+BNET_API int bnet_ema_advance(BnetColl* c, float* blk, void* stream) {
+  if (ema_block_check(blk) < 0) return -1;
+  return launch(bnet_ema_advance_kernel, 1, 1, (cudaStream_t)stream, blk);
 }
 
 BNET_API int bnet_pack_cast(const BnetPackItem* items_dev, int n, void* dst, int src_dtype, int dst_dtype, float scale,

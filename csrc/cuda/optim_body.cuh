@@ -1,6 +1,6 @@
 // Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu): sgd_update for
-// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, clip_coef for the clipped step, and lars_trust /
-// lars_scalars for the LARS step.
+// bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, clip_coef for the clipped step, lars_trust /
+// lars_scalars for the LARS step, and ema_gate / ema_lerp for the EMA of the master weights.
 //
 // The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
 // kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks SGD and AdamW against long-double
@@ -117,6 +117,31 @@ BNET_OPT_HD LarsScalars lars_scalars(float eta, float eps, float wd, float gs, f
 // The first four are the SGD block's {lr, momentum, weight_decay, grad_scale}.
 enum { kLarsLr = 0, kLarsMomentum, kLarsWeightDecay, kLarsGradScale, kLarsEta, kLarsEps, kLarsReserved0, kLarsReserved1,
        kLarsWords };
+
+// Device block of the exponential moving average of the master weights: 4 floats, 16-byte aligned.  `weight` is
+// 1 - decay, computed in double by the host and rounded once, which is the fp32 weight torch._foreach_lerp_ gets from
+// torch.optim.swa_utils.get_ema_multi_avg_fn(decay).  `step` counts the optimizer steps taken and `n_averaged` the EMA
+// updates, as AveragedModel.n_averaged; both are advanced on the device (bnet_ema_advance_kernel), so a captured CUDA
+// graph keeps counting.  A float counts exactly up to 2^24 steps.
+enum { kEmaWeight = 0, kEmaEvery, kEmaStep, kEmaNAveraged, kEmaWords };
+
+// Whether the optimizer step about to be counted (step + 1, steps counted from 1) updates the EMA, and whether that
+// update is a copy (no update averaged yet, as AveragedModel's n_averaged == 0).  `every` >= 1.
+struct EmaGate {
+  bool update, copy;
+};
+BNET_OPT_HD EmaGate ema_gate(float step, float every, float n_averaged) {
+  const bool update = ((unsigned)step + 1u) % (unsigned)every == 0u;
+  return {update, update && n_averaged == 0.0f};
+}
+
+// torch.lerp(ema, w, weight) in fp32: ema + weight*(w - ema) for |weight| < 0.5, else w - (w - ema)*(1 - weight).  The
+// second branch makes weight = 1 give w exactly.  NaN and Inf follow IEEE arithmetic as in torch's kernel: a NaN in
+// either operand gives NaN, and ema = +-Inf with w finite gives NaN (Inf - Inf) in the first branch.
+BNET_OPT_HD float ema_lerp(float ema, float w, float weight) {
+  const float d = w - ema;
+  return fabsf(weight) < 0.5f ? fmaf(weight, d, ema) : fmaf(-d, 1.0f - weight, w);
+}
 
 }  // namespace optim
 }  // namespace bnet

@@ -1,7 +1,7 @@
 // CPU test of the fused optimizer updates: compiles the per-element bodies of csrc/cuda/optim_body.cuh (what
 // bnet_fused_adamw_kernel and bnet_fused_sgd_kernel inline) with g++ and compares them with a long-double AdamW and SGD
 // fed the same fp32 inputs and the same fp32 hyper-parameters.  The SGD part and its bound are further down, and so is
-// the LARS trust ratio (lars_trust / lars_scalars).
+// the LARS trust ratio (lars_trust / lars_scalars) and the EMA gate and lerp (ema_gate / ema_lerp).
 //
 // AdamW:
 // Bound (u = 2^-24, F = 4 * 2^-149 for results in the subnormal range).  With M = b1|m| + (1-b1)|g|,
@@ -298,15 +298,89 @@ static void lars_checks() {
   CHECK(e.t == 1.f && isnan(e.gscale) && e.wd == 0.f, "excluded tensor keeps a NaN clip coefficient in its scale");
 }
 
+// ---------------------------------------------------------------------------------------------------------- EMA
+// ema_gate against integer arithmetic: step s + 1 updates when (s + 1) % every == 0, and the update is a copy when
+// n_averaged == 0, for counters up to 2^24.  ema_lerp against torch.lerp's two branches in long double on the same fp32
+// inputs: the difference and the fma round once each, so to first order |r - R| <= u(|R| + min(w, 1 - w)|m - e|) (+ F,
+// and a factor 1 + 2^-13 for the second-order term); weight 0 gives
+// the EMA and weight 1 the master exactly; NaN and +-Inf give what the same formula gives in IEEE arithmetic.
+static double e_worst = 0.0;
+
+static LD lerp_ref(float e, float m, float w) {
+  const LD d = (LD)m - (LD)e;
+  return fabsf(w) < 0.5f ? (LD)e + (LD)w * d : (LD)m - d * (1.0L - (LD)w);
+}
+
+static void ema_checks() {
+  const unsigned everys[] = {1u, 2u, 3u, 7u, 32u, 1000u, 1u << 12, (1u << 23) + 1u, 1u << 23, 1u << 24};
+  const unsigned steps[] = {0u, 1u, 2u, 6u, 30u, 31u, 32u, 999u, 4095u, 4096u, (1u << 23) - 1u, 1u << 23,
+                            (1u << 24) - 2u, (1u << 24) - 1u};
+  const float counts[] = {0.f, 1.f, 5.f, 16777216.f};
+  for (const unsigned ev : everys)
+    for (const unsigned s : steps)
+      for (const float n : counts) {
+        const EmaGate g = ema_gate((float)s, (float)ev, n);
+        const bool due = (s + 1u) % ev == 0u;
+        CHECK(g.update == due && g.copy == (due && n == 0.f), "ema_gate(step=%u, every=%u, n=%g) = {%d, %d}", s, ev, n,
+              g.update, g.copy);
+      }
+  // a run of steps from 0, counting as bnet_ema_advance_kernel does
+  const unsigned runs[] = {1u, 3u, 32u};
+  for (const unsigned ev : runs) {
+    float step = 0.f, n = 0.f;
+    unsigned updates = 0, copies = 0;
+    for (unsigned s = 1; s <= 1000; s++) {
+      const EmaGate g = ema_gate(step, (float)ev, n);
+      updates += g.update, copies += g.copy;
+      if (g.update) n += 1.f;
+      step += 1.f;
+    }
+    CHECK(updates == 1000 / ev && copies == 1 && n == (float)(1000 / ev) && step == 1000.f, "every=%u: %u updates, %u copies",
+          ev, updates, copies);
+  }
+  const float weights[] = {0.f, 1.f, 2e-5f, 3.0517578e-4f, 1e-3f, 0.1f, 0.4999999f, 0.5f, 0.5000001f, 0.75f, 0.999f};
+  for (const float w : weights)
+    for (int i = 0; i < 20000; i++) {
+      // EMA and master close to each other (the usual case), far apart, and of different magnitudes
+      const float scale = ldexpf(1.f, (int)(urand() * 40.f) - 20);
+      const float e = srand_(scale);
+      const float m = (i & 1) ? e + srand_(scale * 1e-3f) : srand_(scale * ((i & 2) ? 1.f : 1e4f));
+      const float r = ema_lerp(e, m, w);
+      if (w == 0.f) { CHECK(r == e, "weight 0: %g, not the EMA %g", r, e); continue; }
+      if (w == 1.f) { CHECK(r == m, "weight 1: %g, not the master %g", r, m); continue; }
+      const LD R = lerp_ref(e, m, w);
+      const LD bound = (1 + ldexpl(1.0L, -13)) * kU * (fabsl(R) + fminl((LD)w, 1.0L - (LD)w) * fabsl((LD)m - (LD)e)) + kF;
+      const LD err = fabsl((LD)r - R);
+      CHECK(isfinite(r) && err <= bound, "ema_lerp(%g, %g, %g) = %.9g, reference %.12Lg", e, m, w, r, R);
+      if (bound > 0 && (double)(err / bound) > e_worst) e_worst = (double)(err / bound);
+    }
+  // NaN and +-Inf in either operand, in both branches
+  const float specials[] = {NAN, INFINITY, -INFINITY, 0.5f};
+  const float sweights[] = {0.f, 1e-3f, 0.75f, 1.f};
+  for (const float w : sweights)
+    for (const float e : specials)
+      for (const float m : specials) {
+        const float r = ema_lerp(e, m, w);
+        const LD R = lerp_ref(e, m, w);
+        CHECK(isnan(R) ? isnan(r) : (LD)r == R, "ema_lerp(%g, %g, %g) = %g, reference %Lg", e, m, w, r, R);
+      }
+  CHECK(isnan(ema_lerp(INFINITY, 1.f, 1e-3f)), "EMA +inf, finite master, small weight: inf - inf = NaN, as torch.lerp");
+  CHECK(ema_lerp(1.f, INFINITY, 1e-3f) == INFINITY, "an infinite master makes the EMA infinite below weight 0.5");
+  CHECK(isnan(ema_lerp(1.f, INFINITY, 0.75f)), "... and NaN above it (inf - inf * (1 - w)), as torch.lerp");
+}
+
 int main() {
+  ema_checks();
+  const int ema = g_checks;
+  printf("optim_emu_test: ema %d checks, worst error/bound %.3f\n", ema, e_worst);
   lars_checks();
-  const int lars = g_checks;
+  const int lars = g_checks - ema;
   printf("optim_emu_test: lars %d checks, worst error/bound %.3f\n", lars, l_worst);
   adamw_checks();
-  const int adamw = g_checks - lars;
+  const int adamw = g_checks - lars - ema;
   printf("optim_emu_test: adamw %d checks, worst error/bound %.3f\n", adamw, g_worst);
   sgd_checks();
-  printf("optim_emu_test: sgd %d checks, worst error/bound %.3f\n", g_checks - adamw - lars, s_worst);
+  printf("optim_emu_test: sgd %d checks, worst error/bound %.3f\n", g_checks - adamw - lars - ema, s_worst);
   printf("optim_emu_test: %d checks, %d failures\n", g_checks, g_fail);
   if (g_fail) return 1;
   printf("optim_emu_test: ok\n");

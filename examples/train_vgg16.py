@@ -23,20 +23,39 @@ def main():
     ap.add_argument("--batch", type=int, default=32, help="images per rank and optimizer step")
     ap.add_argument("--accumulation-steps", type=int, default=1,
                     help="split every batch into this many micro-batches (one forward/backward each) and update once")
+    ap.add_argument("--ema-decay", type=float, default=None,
+                    help="keep an exponential moving average of the weights with this decay (torchvision uses 0.99998)")
+    ap.add_argument("--ema-every", type=int, default=1, help="update the EMA after every this many optimizer steps")
     ap.add_argument("--model", default="vgg16")
     ap.add_argument("--checkpoint", default="")
     a = ap.parse_args()
     init_process_group_from_env()
     rank = int(os.environ.get("RANK", "0"))
     model = build_model(a.model, fused=True).cuda().bfloat16().to(memory_format=torch.channels_last)
-    engine = BnetDDP(model, lr=0.01, momentum=0.9, weight_decay=1e-4, accumulation_steps=a.accumulation_steps)
+    engine = BnetDDP(model, lr=0.01, momentum=0.9, weight_decay=1e-4, accumulation_steps=a.accumulation_steps,
+                     ema_decay=a.ema_decay, ema_every=a.ema_every)
     engine.enable_cuda_graph(True)            # forward + backward + every bucket kernel replay as one graph
     engine.set_lr(0.01)                       # hyper-parameters live in device memory: the graph follows the schedule
-    for step, loss in enumerate(engine.train_from_host(batches(a.steps, a.batch, rank))):
+    last = []
+
+    def remember(it):                         # (the last batch, for the evaluation on the EMA weights below)
+        for b in it:
+            last[:] = [b]
+            yield b
+
+    for step, loss in enumerate(engine.train_from_host(remember(batches(a.steps, a.batch, rank)))):
         if step % 10 == 0:
             engine.set_lr(0.01 * 0.5 ** (step // 20))
             if rank == 0:
                 print(f"step {step:4d}  loss {float(loss):.4f}")
+    if a.ema_decay is not None and last:
+        x, y = last[0][0].cuda().contiguous(memory_format=torch.channels_last), last[0][1].cuda()
+        model.eval()
+        with engine.ema_parameters(), torch.no_grad():    # every rank takes part
+            ema_loss = float(torch.nn.functional.cross_entropy(model(x).float(), y))
+        model.train()
+        if rank == 0:
+            print(f"last batch on the EMA weights: loss {ema_loss:.4f}")
     if a.checkpoint and rank == 0:
         torch.save({"model": model.state_dict(), "optimizer": engine.optimizer_state_dict()}, a.checkpoint)
 

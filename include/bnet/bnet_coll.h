@@ -175,6 +175,20 @@ int bnet_fused_lars_apply(BnetColl* c, size_t param_off, size_t count, int dtype
                           int nseg, const float* scal, const float* hp, float* master, float* mom_buf, int channel, int nblocks,
                           void* stream);
 
+/* Exponential moving average (EMA) of the fp32 master weights, as torch.optim.swa_utils.AveragedModel with
+ * get_ema_multi_avg_fn(decay) and use_buffers=False, applied to this rank's master shards.  The EMA block is 4 floats of
+ * device memory, 16-byte aligned: {weight = 1 - decay, every, step, n_averaged} (csrc/cuda/optim_body.cuh).  `step`
+ * counts the optimizer steps taken; step s (counted from 1) is an EMA step when s % every == 0.  Counters are floats,
+ * exact up to 2^24.
+ *
+ * Per bucket, after the optimizer step's last update: on an EMA step, ema = master when n_averaged == 0, else
+ * ema = torch.lerp(ema, master, weight), over `count` floats (a whole number of float4s, both shards 16-byte aligned);
+ * on any other step the kernel reads the block and exits.  Rank-local, deterministic, no barriers. */
+int bnet_ema_update(BnetColl* c, size_t count, const float* master, float* ema, const float* blk, int nblocks, void* stream);
+/* Once per optimizer step, after every bucket's bnet_ema_update: n_averaged += 1 on an EMA step, then step += 1.  One
+ * thread. */
+int bnet_ema_advance(BnetColl* c, float* blk, void* stream);
+
 /* Multi-tensor pack+cast into the heap (K5): n tensors described on the device. */
 typedef struct {
   const void* src;

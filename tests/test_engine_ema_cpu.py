@@ -1,0 +1,388 @@
+"""BnetDDP(ema_decay=...)'s HOST logic on the CPU: the EMA of the master weights against a float64
+torch.optim.swa_utils.AveragedModel (SGD, AdamW and LARS, every 1 and 3, k = 1 and 2, clipped and unclipped), a bucket
+without gradient, set_ema_decay and reset_ema mid-run, the launch order, ema_parameters(), the state dict and its
+cross-loading rules, an engine without EMA, and every rejected argument.  The comm below does the kernels' work in plain
+PyTorch; the kernels are covered on the GPU by tests/test_ema.py."""
+import copy
+import math
+
+import pytest
+import torch
+from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import small_model as _model
+from torch.optim.swa_utils import AveragedModel, get_ema_multi_avg_fn
+
+from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_lars_segments, check_lars_tensors
+from bagua_net_b200.parallel.ddp import BnetDDP
+
+
+class EmaComm(FakeComm):
+    """FakeComm plus the staged step, the LARS stages and the two EMA kernels; `log` lists every call in order."""
+
+    def __init__(self):
+        super().__init__()
+        self.log = []
+
+    def fused_allreduce_sgd(self, grad, *a, **k):
+        self.log.append(("update", grad.numel()))
+        super().fused_allreduce_sgd(grad, *a, **k)
+
+    def fused_allreduce_adamw(self, grad, *a, **k):
+        self.log.append(("update", grad.numel()))
+        super().fused_allreduce_adamw(grad, *a, **k)
+
+    def _stage1(self, kind, grad, scratch, partial, add):
+        assert partial.numel() == CLIP_ROW
+        scratch.add_(grad.float()) if add else scratch.copy_(grad.float())
+        partial.zero_()
+        partial[0] = scratch.double().square().sum()
+        grad.zero_()
+        self.launches += 1
+        self.log.append((kind, grad.numel()))
+
+    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
+        self._stage1("norm", grad, scratch, partial, add=False)
+
+    def fused_accum_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
+        self._stage1("accum", grad, scratch, partial, add=True)
+
+    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
+        total = torch.tensor(math.sqrt(float(partials.sum())) * grad_scale, dtype=torch.float32)
+        clip[1] = total
+        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
+        self.launches += 1
+        self.log.append(("coef", None))
+
+    def barrier(self, channel=2, stream=None):
+        self.log.append(("barrier", None))
+
+    def fused_clip_apply_sgd(self, param, scratch, clip, master, mom, lr, momentum, weight_decay, grad_scale=None, channel=0,
+                             nblocks=0, stream=None, hp=None):
+        self.log.append(("update", param.numel()))
+        FakeComm.fused_allreduce_sgd(self, scratch * clip[2], param, master, mom, lr, momentum, weight_decay, grad_scale,
+                                     zero_grads=False, hp=hp)
+
+    def fused_clip_apply_adamw(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, channel=0, nblocks=0, stream=None):
+        self.log.append(("update", param.numel()))
+        FakeComm.fused_allreduce_adamw(self, scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, zero_grads=False)
+
+    def lars_segments(self, table, shard_vecs, ntensors):
+        check_lars_segments(table, shard_vecs, ntensors)
+        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
+
+    def lars_tensors(self, table, nslots):
+        check_lars_tensors(table, nslots)
+        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
+
+    def fused_lars_norm(self, master, scratch, segs, slots, dtype, nblocks=0, stream=None):
+        e = 16 // torch.empty((), dtype=dtype).element_size()
+        for vec0, nvec, _, slot0 in segs.tolist():
+            for c in range((nvec + LARS_CHUNK - 1) // LARS_CHUNK):
+                a, b = (vec0 + c * LARS_CHUNK) * e, (vec0 + min(nvec, (c + 1) * LARS_CHUNK)) * e
+                slots[slot0 + c] = torch.stack([master[a:b].double().square().sum(), scratch[a:b].double().square().sum()])
+        self.launches += 1
+        self.log.append(("lars_norm", master.numel()))
+
+    def fused_lars_trust(self, slots, tensors, xchg, clip, hp, scal, trust, channel=0, stream=None):
+        f = lambda v: torch.tensor(float(v), dtype=torch.float32)  # noqa: E731
+        gscale, wd, eta, eps, coef = f(hp[3]), f(hp[2]), f(hp[4]), f(hp[5]), f(clip[2])
+        for j, (slot0, n, excluded, _) in enumerate(tensors.tolist()):
+            w2, g2 = (float(v) for v in slots[slot0:slot0 + n].sum(0)) if n else (0.0, 0.0)
+            wn, gn = f(math.sqrt(w2)), f(math.sqrt(g2) * float(gscale) * float(coef))
+            live = not excluded and wn != 0 and gn != 0
+            t = eta * wn / (gn + wd * wn + eps) if live else torch.tensor(1.0)
+            scal[j, 0], scal[j, 1], trust[j] = gscale * coef * t, wd * t if live else 0.0, t
+        self.launches += 1
+        self.log.append(("lars_trust", None))
+
+    def fused_lars_apply(self, param, scratch, segs, scal, hp, master, mom, channel=0, nblocks=0, stream=None):
+        lr, mu = float(hp[0]), float(hp[1])
+        e = 16 // param.element_size()
+        for vec0, nvec, tensor, _ in segs.tolist():
+            s = slice(vec0 * e, (vec0 + nvec) * e)
+            mom[s].mul_(mu).add_(scratch[s] * scal[tensor, 0] + scal[tensor, 1] * master[s])
+            master[s].sub_(lr * mom[s])
+        param.copy_(master.to(param.dtype))
+        self.launches += 1
+        self.log.append(("update", param.numel()))
+
+    # the EMA kernels: the gate of optim::ema_gate on the block {1 - decay, every, step, n_averaged}, torch.lerp
+    def ema_update(self, master, ema, blk, nblocks=0, stream=None):
+        assert blk.dtype == torch.float32 and blk.numel() == 4 and ema.shape == master.shape
+        w, every, step, n = blk.tolist()
+        if (int(step) + 1) % int(every) == 0:
+            ema.copy_(master if n == 0 else torch.lerp(ema, master, w))
+        self.launches += 1
+        self.log.append(("ema_update", master.numel()))
+
+    def ema_advance(self, blk, stream=None):
+        w, every, step, n = blk.tolist()
+        if (int(step) + 1) % int(every) == 0:
+            blk[3] += 1
+        blk[2] += 1
+        self.launches += 1
+        self.log.append(("ema_advance", None))
+
+
+BATCH = 8
+HYPER = {"sgd": dict(lr=0.05, momentum=0.9, weight_decay=1e-3),
+         "adamw": dict(lr=3e-3, betas=(0.85, 0.99), eps=1e-7, weight_decay=0.05),
+         "lars": dict(lr=0.5, momentum=0.9, weight_decay=5e-4, trust_coefficient=0.02, eps=1e-8)}
+DECAY = 0.6                  # weights 0.4 (the lerp's first branch) and, after set_ema_decay(0.3), 0.7 (its second)
+
+
+def _batch(step):
+    torch.manual_seed(300 + step)
+    return torch.randn(BATCH, 3, 8, 8).contiguous(memory_format=torch.channels_last), torch.randint(0, 10, (BATCH,))
+
+
+def _engine(net, optimizer="sgd", **kw):
+    return BnetDDP(net, optimizer=optimizer, bucket_mb=0.002, comm=EmaComm(), **HYPER[optimizer], **kw)
+
+
+def _reference(ref, optimizer):
+    h = HYPER[optimizer]
+    if optimizer == "adamw":
+        return torch.optim.AdamW(ref.parameters(), **h)
+    return torch.optim.SGD(ref.parameters(), lr=h["lr"], momentum=h["momentum"],
+                           weight_decay=0.0 if optimizer == "lars" else h["weight_decay"])
+
+
+def _ref_step(ref, opt, optimizer, x, y, k, max_norm):
+    """One optimizer step of the float64 reference on the global batch (k micro-batches, clipped when max_norm)."""
+    opt.zero_grad()
+    for xs, ys in zip(x.split(BATCH // k), y.split(BATCH // k)):
+        (torch.nn.functional.cross_entropy(ref(xs.double()), ys) / k).backward()
+    if max_norm is not None:
+        torch.nn.utils.clip_grad_norm_(ref.parameters(), max_norm)
+    if optimizer == "lars":                               # Apex LARC(clip=False) in front of SGD
+        h = HYPER["lars"]
+        with torch.no_grad():
+            for p in ref.parameters():
+                if p.grad is None or p.dim() <= 1:
+                    continue
+                wn, gn = p.norm(), p.grad.norm()
+                if wn != 0 and gn != 0:
+                    p.grad.add_(p, alpha=h["weight_decay"]).mul_(h["trust_coefficient"] * wn / (gn + wn * h["weight_decay"] + h["eps"]))
+    opt.step()
+
+
+def _flat_ema(eng):
+    return torch.cat([b.ema for b in eng.buckets])        # (one rank: the shards are the buckets, in flat order)
+
+
+def _as_params(eng, net, flat):
+    """`flat` (laid out as flat_param) as one tensor per parameter of `net`."""
+    base, es = eng.flat_param.data_ptr(), eng.flat_param.element_size()
+    return [flat.as_strided(p.shape, p.stride(), (p.data_ptr() - base) // es) for p in net.parameters()]
+
+
+def _ema_f64(ema, master, decay, n):
+    return master.clone() if n == 0 else torch.lerp(ema, master, 1.0 - decay)
+
+
+@pytest.mark.parametrize("k", [1, 2])
+@pytest.mark.parametrize("every", [1, 3])
+@pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
+@pytest.mark.parametrize("optimizer", ["sgd", "adamw", "lars"])
+def test_ema_matches_averaged_model(cpu_engine, optimizer, clipped, every, k):
+    thr = 0.05 if clipped else None
+    ref, net = _model().double(), _model()
+    opt = _reference(ref, optimizer)
+    avg = AveragedModel(ref, multi_avg_fn=get_ema_multi_avg_fn(DECAY), use_buffers=False)
+    eng = _engine(net, optimizer, ema_decay=DECAY, ema_every=every, max_grad_norm=thr, accumulation_steps=k)
+    assert len(eng.buckets) >= 2
+    assert torch.equal(_flat_ema(eng), torch.cat([b.master for b in eng.buckets]))   # a copy of the masters at first
+    own = _flat_ema(eng).double()                          # float64 EMA of the engine's own masters
+    n = 0
+    for step in range(1, 8):
+        x, y = _batch(step)
+        _ref_step(ref, opt, optimizer, x, y, k, thr)
+        eng.train_step(x, y)
+        if step % every == 0:
+            avg.update_parameters(ref)
+            own = _ema_f64(own, torch.cat([b.master for b in eng.buckets]).double(), DECAY, n)
+            n += 1
+        assert eng._ema.tolist() == [pytest.approx(1 - DECAY), every, step, n]
+        got = _flat_ema(eng)
+        assert torch.allclose(got.double(), own, rtol=0, atol=4 * 2.0 ** -24 * float(own.abs().max())), step
+        for a, b in zip(_as_params(eng, net, got), avg.module.parameters()):
+            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5), (step, float((a.double() - b).abs().max()))
+    assert int(avg.n_averaged) == n == 7 // every
+
+
+class _Branchy(torch.nn.Module):
+    def __init__(self, channels_last=True):
+        super().__init__()
+        torch.manual_seed(4)
+        self.unused = torch.nn.Linear(32, 32, bias=False)
+        self.net = _model(channels_last)
+
+    def forward(self, x):
+        return self.net(x)
+
+
+@pytest.mark.parametrize("optimizer", ["sgd", "lars"])
+def test_bucket_without_gradient_updates_its_ema(cpu_engine, optimizer):
+    net = _Branchy()
+    eng = _engine(net, optimizer, ema_decay=DECAY)
+    idle = [b for b in eng.buckets if len(b.params) == 1 and b.params[0] is net.unused.weight]
+    assert len(idle) == 1
+    idle = idle[0]
+    eng.train_step(*_batch(0))                             # the copy step
+    assert torch.equal(idle.ema, idle.master)
+    idle.ema.zero_()
+    eng.train_step(*_batch(1))                             # lerp(0, master, 0.4): the bucket's EMA moves without a gradient
+    assert torch.equal(idle.ema, torch.lerp(torch.zeros_like(idle.master), idle.master, float(eng._ema[0])))
+    assert [kind for kind, _ in eng.comm.log].count("ema_update") == 2 * len(eng.buckets)
+
+
+def test_set_ema_decay_and_reset_ema_mid_run(cpu_engine):
+    ref, net = _model().double(), _model()
+    opt = _reference(ref, "sgd")
+    avg = AveragedModel(ref, multi_avg_fn=get_ema_multi_avg_fn(DECAY), use_buffers=False)
+    eng = _engine(net, ema_decay=DECAY, ema_every=2)
+    for step in range(1, 11):
+        if step == 4:                                      # a decay schedule: weight 0.7, the lerp's other branch
+            eng.set_ema_decay(0.3)
+            avg.multi_avg_fn = get_ema_multi_avg_fn(0.3)
+        if step == 7:                                      # torchvision's n_averaged.fill_(0): the next update copies
+            eng.reset_ema()
+            avg.n_averaged.fill_(0)
+        x, y = _batch(step)
+        _ref_step(ref, opt, "sgd", x, y, 1, None)
+        eng.train_step(x, y)
+        if step % 2 == 0:
+            avg.update_parameters(ref)
+        if step == 8:
+            assert torch.equal(_flat_ema(eng), torch.cat([b.master for b in eng.buckets]))   # the copy after the reset
+        for a, b in zip(_as_params(eng, net, _flat_ema(eng)), avg.module.parameters()):
+            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5), step
+    assert eng._ema.tolist() == [pytest.approx(0.7), 2, 10, 2] and int(avg.n_averaged) == 2
+    assert eng.ema_decay == 0.3
+
+
+@pytest.mark.parametrize("k", [1, 2])
+@pytest.mark.parametrize("kind", ["sgd", "adamw", "lars", "sgd-clipped"])
+def test_launch_order(cpu_engine, kind, k):
+    optimizer = kind.split("-")[0]
+    eng = _engine(_model(), optimizer, ema_decay=DECAY, ema_every=2, accumulation_steps=k,
+                  max_grad_norm=1.0 if "clipped" in kind else None)
+    nb, comm = len(eng.buckets), eng.comm
+    for step in range(3):
+        n0, l0 = len(comm.log), comm.launches
+        eng.train_step(*_batch(step))
+        kinds = [kind for kind, _ in comm.log[n0:]]
+        last = max(i for i, kd in enumerate(kinds) if kd == "update")
+        assert kinds.count("update") == nb                   # one optimizer step per train_step ...
+        assert kinds[last + 1:] == ["ema_update"] * nb + ["ema_advance"]   # ... then the EMA, on every step
+        assert [n for kd, n in comm.log[n0:] if kd == "ema_update"] == [b.master.numel() for b in eng.buckets]
+        assert comm.launches - l0 == len([kd for kd in kinds if kd != "barrier"])
+    assert eng._ema.tolist()[2:] == [3, 1]
+
+
+def test_ema_parameters_publishes_and_restores(cpu_engine):
+    for dtype in (torch.float32, torch.bfloat16):
+        net = _model().to(dtype)
+        eng = _engine(net, ema_decay=DECAY, accumulation_steps=2)
+        if dtype == torch.float32:
+            for step in range(3):
+                eng.train_step(*_batch(step))
+        torch.manual_seed(9)
+        for b in eng.buckets:                              # an EMA away from the masters, below a bf16 ulp too
+            b.ema.copy_(b.master + torch.randn_like(b.master) * 1e-3)
+        before = eng.flat_param.clone()
+        with eng.ema_parameters() as m:
+            assert m is net
+            assert torch.equal(eng.flat_param, _flat_ema(eng).to(dtype))
+            for p, e in zip(net.parameters(), _as_params(eng, net, _flat_ema(eng))):
+                assert torch.equal(p.detach(), e.to(dtype))
+            with pytest.raises(ValueError):
+                eng.train_step(*_batch(0))
+            with pytest.raises(ValueError):
+                eng.finish_step()
+            with pytest.raises(ValueError):
+                with eng.ema_parameters():
+                    pass
+        assert torch.equal(eng.flat_param.view(torch.uint8), before.view(torch.uint8))
+        if dtype == torch.float32:                         # in the middle of an accumulation step
+            x, y = _batch(5)
+            torch.nn.functional.cross_entropy(net(x[:4]), y[:4]).backward()
+            eng.finish_step()
+            assert eng.micro_step == 1
+            with pytest.raises(ValueError):
+                with eng.ema_parameters():
+                    pass
+    with pytest.raises(ValueError):
+        with _engine(_model()).ema_parameters():
+            pass
+
+
+SGD_KEYS = {"lr", "momentum", "weight_decay", "world", "rank", "buckets"}
+EMA_KEYS = {"ema_decay", "ema_every", "ema_step", "ema_n_averaged"}
+
+
+@pytest.mark.parametrize("optimizer", ["sgd", "adamw", "lars"])
+def test_state_dict_round_trip(cpu_engine, optimizer):
+    eng = _engine(_model(), optimizer, ema_decay=DECAY, ema_every=2)
+    for step in range(5):
+        eng.train_step(*_batch(step))
+    state = eng.optimizer_state_dict()
+    plain = set(_engine(_model(), optimizer).optimizer_state_dict())
+    assert set(state) == plain | EMA_KEYS
+    assert (state["ema_decay"], state["ema_every"], state["ema_step"], state["ema_n_averaged"]) == (DECAY, 2, 5, 2)
+    assert all("ema" in b and torch.equal(b["ema"], e.ema) for b, e in zip(state["buckets"], eng.buckets))
+    resumed = _engine(_model(), optimizer, ema_decay=0.9, ema_every=5)
+    resumed.load_optimizer_state_dict(copy.deepcopy(state))
+    assert torch.equal(resumed._ema, eng._ema) and (resumed.ema_decay, resumed.ema_every) == (DECAY, 2)
+    for b1, b2 in zip(resumed.buckets, eng.buckets):
+        assert torch.equal(b1.ema, b2.ema) and all(torch.equal(t1, t2) for t1, t2 in zip(b1.state, b2.state))
+
+
+def test_state_dict_cross_loading(cpu_engine):
+    with_ema = _engine(_model(), ema_decay=DECAY)
+    without = _engine(_model())
+    for step in range(2):
+        with_ema.train_step(*_batch(step))
+        without.train_step(*_batch(step))
+    # an EMA would be dropped silently: refused, and nothing is loaded
+    masters = [b.master.clone() for b in without.buckets]
+    with pytest.raises(ValueError):
+        without.load_optimizer_state_dict(copy.deepcopy(with_ema.optimizer_state_dict()))
+    assert all(torch.equal(m, b.master) for m, b in zip(masters, without.buckets))
+    # a plain checkpoint into an engine with an EMA: the EMA restarts from the loaded masters
+    target = _engine(_model(), ema_decay=DECAY)
+    target.load_optimizer_state_dict(copy.deepcopy(without.optimizer_state_dict()))
+    for b, o in zip(target.buckets, without.buckets):
+        assert torch.equal(b.master, o.master) and torch.equal(b.ema, o.master)
+    assert target._ema.tolist() == [pytest.approx(1 - DECAY), 1, 0, 0]
+
+
+def test_engine_without_ema_is_unchanged(cpu_engine):
+    eng = _engine(_model())
+    assert eng.ema_decay is None and eng._ema is None and all(b.ema is None for b in eng.buckets)
+    for step in range(2):
+        n0, l0 = len(eng.comm.log), eng.comm.launches
+        eng.train_step(*_batch(step))
+        assert [kind for kind, _ in eng.comm.log[n0:]] == ["update"] * len(eng.buckets)
+        assert eng.comm.launches - l0 == len(eng.buckets)
+    state = eng.optimizer_state_dict()
+    assert set(state) == SGD_KEYS and all(set(b) == {"master", "momentum"} for b in state["buckets"])
+    for call in (lambda: eng.set_ema_decay(0.9), eng.reset_ema):
+        with pytest.raises(ValueError):
+            call()
+
+
+def test_rejects_bad_arguments(cpu_engine):
+    for bad in ({"ema_decay": -0.1}, {"ema_decay": 1.5}, {"ema_decay": float("nan")}, {"ema_decay": float("inf")},
+                {"ema_decay": "x"}, {"ema_decay": [0.9]}, {"ema_decay": 0.9, "ema_every": 0},
+                {"ema_decay": 0.9, "ema_every": -3}, {"ema_decay": 0.9, "ema_every": 2.0}, {"ema_decay": 0.9, "ema_every": True},
+                {"ema_decay": 0.9, "ema_every": "2"}, {"ema_decay": 0.9, "ema_every": (1 << 24) + 1}):
+        with pytest.raises(ValueError):
+            _engine(_model(), **bad)
+    eng = _engine(_model(), ema_decay=0.0)               # the ends of [0, 1] are allowed
+    _engine(_model(), ema_decay=1, ema_every=1 << 24)
+    for bad in (-1e-9, 1.0000001, float("nan"), None):
+        with pytest.raises(ValueError):
+            eng.set_ema_decay(bad)
+    assert eng.ema_decay == 0.0 and float(eng._ema[0]) == 1.0
