@@ -2,7 +2,7 @@
 contribution in the step, add after that), once per step the coefficient (clipping) or a barrier, one update per bucket,
 1/(world * k) gradient scaling, AdamW's step count, micro_step, the custom backward + finish_step loop, and the arguments
 and calls it rejects.  The reference is a float64 copy of the model trained by torch.optim.SGD / AdamW on the FULL batch
-(+ clip_grad_norm_).  The comm below does the stages in plain PyTorch; the kernels are covered on the GPU by
+(+ clip_grad_norm_).  FakeComm does the stages in plain PyTorch; the kernels are covered on the GPU by
 tests/test_grad_accum.py."""
 import copy
 import math
@@ -12,71 +12,7 @@ import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
 from engine_fakes import small_model as _model
 
-from bagua_net_b200.parallel.comm import CLIP_ROW
 from bagua_net_b200.parallel.ddp import BnetDDP
-
-
-class AccumComm(FakeComm):
-    """FakeComm plus the staged step: store, accumulate, coefficient, barrier and apply; `log` lists every call in order."""
-
-    def __init__(self):
-        super().__init__()
-        self.log = []
-        self.coef_scales = []              # the gradient scale of every coefficient launch
-        self.apply_scales = []             # ... and of every update from the scratch
-
-    def fused_allreduce_sgd(self, grad, *a, **k):
-        self.log.append(("sgd", grad.numel()))
-        super().fused_allreduce_sgd(grad, *a, **k)
-
-    def fused_allreduce_adamw(self, grad, *a, **k):
-        self.log.append(("adamw", grad.numel()))
-        super().fused_allreduce_adamw(grad, *a, **k)
-
-    def _stage1(self, kind, grad, scratch, partial, add):
-        assert scratch.dtype == torch.float32 and scratch.numel() * self.world == grad.numel()
-        assert partial.dtype == torch.float64 and partial.numel() == CLIP_ROW
-        if add:
-            scratch.add_(grad.float())
-        else:
-            scratch.copy_(grad.float())
-        partial.zero_()
-        partial[0] = scratch.double().square().sum()         # over the (new) scratch values
-        grad.zero_()
-        self.launches += 1
-        self.log.append((kind, grad.numel()))
-
-    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("norm", grad, scratch, partial, add=False)
-
-    def fused_accum_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("accum", grad, scratch, partial, add=True)
-
-    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
-        assert partials.shape[1] == CLIP_ROW and xchg.numel() >= self.world and clip.numel() == 4
-        gs = 1.0 / self.world if grad_scale is None else grad_scale
-        self.coef_scales.append(gs)
-        total = torch.tensor(math.sqrt(float(partials.sum())) * gs, dtype=torch.float32)
-        clip[1] = total
-        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
-        self.launches += 1
-        self.log.append(("coef", partials.shape[0]))
-
-    def barrier(self, channel=2, stream=None):
-        assert channel == 0
-        self.log.append(("barrier", None))       # (no kernel on one rank, as SymmComm.barrier)
-
-    def fused_clip_apply_sgd(self, param, scratch, clip, master, mom, lr, momentum, weight_decay, grad_scale=None, channel=0,
-                             nblocks=0, stream=None, hp=None):
-        self.log.append(("apply", param.numel()))
-        self.apply_scales.append(grad_scale if hp is None else float(hp[3]))
-        FakeComm.fused_allreduce_sgd(self, scratch * clip[2], param, master, mom, lr, momentum, weight_decay, grad_scale,
-                                     zero_grads=False, hp=hp)
-
-    def fused_clip_apply_adamw(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, channel=0, nblocks=0, stream=None):
-        self.log.append(("apply", param.numel()))
-        self.apply_scales.append(float(hp[5]))
-        FakeComm.fused_allreduce_adamw(self, scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, zero_grads=False)
 
 
 BATCH = 12                                      # divisible by every k tested
@@ -100,10 +36,10 @@ def _pair(optimizer, channels_last=True, model=None, **kw):
     ref, net = make(channels_last).double(), make(channels_last)
     if optimizer == "adamw":
         opt = torch.optim.AdamW(ref.parameters(), **ADAMW)
-        eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=AccumComm(), **ADAMW, **kw)
+        eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=FakeComm(), **ADAMW, **kw)
     else:
         opt = torch.optim.SGD(ref.parameters(), **SGD)
-        eng = BnetDDP(net, bucket_mb=0.002, comm=AccumComm(), **SGD, **kw)
+        eng = BnetDDP(net, bucket_mb=0.002, comm=FakeComm(), **SGD, **kw)
     return ref, opt, net, eng
 
 
@@ -310,8 +246,8 @@ def test_checkpoint_at_step_boundaries_only(cpu_engine, optimizer):
 def test_rejects_bad_arguments(cpu_engine):
     for bad in (0, -1, 1.5, 2.0, "2", None, True):
         with pytest.raises(ValueError):
-            BnetDDP(_model(), bucket_mb=0.002, comm=AccumComm(), accumulation_steps=bad)
-    eng = BnetDDP(_model(), bucket_mb=0.002, comm=AccumComm(), accumulation_steps=4)
+            BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=bad)
+    eng = BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=4)
     for n in (6, 10, 3):
         x, y = _batch(0, n=n)
         with pytest.raises(ValueError):
@@ -336,6 +272,6 @@ def test_micro_batches_of_a_channels_last_batch_stay_channels_last(cpu_engine):
             seen.append((x.shape[0], x.is_contiguous(memory_format=torch.channels_last)))
             return self.net(x)
 
-    eng = BnetDDP(Spy(), bucket_mb=0.002, comm=AccumComm(), accumulation_steps=3)
+    eng = BnetDDP(Spy(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=3)
     eng.train_step(*_batch(0))
     assert seen == [(4, True)] * 3

@@ -1,8 +1,8 @@
 """BnetDDP(max_grad_norm=...)'s HOST logic on the CPU: the three stages of the clipped step (per bucket reduce + sum of
 squares from the gradient hook, once per step the norm and the coefficient, per bucket the update from the scratch),
 set_max_grad_norm, last_grad_norm, the state dict and the arguments it rejects, against torch.nn.utils.clip_grad_norm_
-followed by torch.optim.SGD / AdamW.  The comm below does the three stages in plain PyTorch; the kernels are covered on
-the GPU by tests/test_grad_clip.py."""
+followed by torch.optim.SGD / AdamW.  FakeComm does the three stages in plain PyTorch; the kernels are covered on the
+GPU by tests/test_grad_clip.py."""
 import copy
 import math
 
@@ -11,53 +11,7 @@ import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
 from engine_fakes import small_model as _model
 
-from bagua_net_b200.parallel.comm import CLIP_ROW
 from bagua_net_b200.parallel.ddp import BnetDDP
-
-
-class ClipComm(FakeComm):
-    """FakeComm plus the clipped step's three stages; `log` lists every call in order."""
-
-    def __init__(self):
-        super().__init__()
-        self.log = []
-
-    def fused_allreduce_sgd(self, grad, *a, **k):
-        self.log.append(("sgd", grad.numel()))
-        super().fused_allreduce_sgd(grad, *a, **k)
-
-    def fused_allreduce_adamw(self, grad, *a, **k):
-        self.log.append(("adamw", grad.numel()))
-        super().fused_allreduce_adamw(grad, *a, **k)
-
-    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        assert scratch.dtype == torch.float32 and scratch.numel() * self.world == grad.numel()
-        assert partial.dtype == torch.float64 and partial.numel() == CLIP_ROW
-        scratch.copy_(grad.float())
-        partial.zero_()
-        partial[0] = scratch.double().square().sum()
-        grad.zero_()
-        self.launches += 1
-        self.log.append(("norm", grad.numel()))
-
-    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
-        assert partials.shape[1] == CLIP_ROW and xchg.numel() >= self.world and clip.numel() == 4
-        gs = 1.0 / self.world if grad_scale is None else grad_scale
-        total = torch.tensor(math.sqrt(float(partials.sum())) * gs, dtype=torch.float32)
-        clip[1] = total
-        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
-        self.launches += 1
-        self.log.append(("coef", partials.shape[0]))
-
-    def fused_clip_apply_sgd(self, param, scratch, clip, master, mom, lr, momentum, weight_decay, grad_scale=None, channel=0,
-                             nblocks=0, stream=None, hp=None):
-        self.log.append(("apply", param.numel()))
-        FakeComm.fused_allreduce_sgd(self, scratch * clip[2], param, master, mom, lr, momentum, weight_decay, grad_scale,
-                                     zero_grads=False, hp=hp)
-
-    def fused_clip_apply_adamw(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, channel=0, nblocks=0, stream=None):
-        self.log.append(("apply", param.numel()))
-        FakeComm.fused_allreduce_adamw(self, scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, zero_grads=False)
 
 
 def _batch(step, channels_last=True):
@@ -76,10 +30,10 @@ def _pair(optimizer, channels_last=True, model=None, **kw):
     ref, net = (model or _model)(channels_last), (model or _model)(channels_last)
     if optimizer == "adamw":
         opt = torch.optim.AdamW(ref.parameters(), **ADAMW)
-        eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=ClipComm(), **ADAMW, **kw)
+        eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=FakeComm(), **ADAMW, **kw)
     else:
         opt = torch.optim.SGD(ref.parameters(), **SGD)
-        eng = BnetDDP(net, bucket_mb=0.002, comm=ClipComm(), **SGD, **kw)
+        eng = BnetDDP(net, bucket_mb=0.002, comm=FakeComm(), **SGD, **kw)
     return ref, net, opt, eng
 
 
@@ -165,8 +119,8 @@ def test_state_dict_keys_are_unchanged(cpu_engine, optimizer):
 def test_rejects_bad_thresholds(cpu_engine):
     for bad in (0.0, -1.0, float("nan"), -math.inf):
         with pytest.raises(ValueError):
-            BnetDDP(_model(), bucket_mb=0.002, comm=ClipComm(), max_grad_norm=bad)
-    eng = BnetDDP(_model(), bucket_mb=0.002, comm=ClipComm(), max_grad_norm=math.inf)
+            BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), max_grad_norm=bad)
+    eng = BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), max_grad_norm=math.inf)
     assert float(eng._clip[0]) == math.inf
     for bad in (0.0, -2.0, float("nan")):
         with pytest.raises(ValueError):

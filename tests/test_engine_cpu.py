@@ -270,3 +270,16 @@ def test_direct_grads_self_check_accepts_the_working_path_and_rejects_a_broken_o
     cpu_engine.setattr(BnetDDP, "_on_grad", broken)
     ok, detail = direct_grads_self_check(**kw)
     assert not ok and "hook failed" in detail["error"]
+
+
+def test_fake_comm_takes_the_parameters_of_symm_comm():
+    """The CPU stand-in is called as the engine calls SymmComm: same parameter names, order and defaults."""
+    import inspect
+
+    from bagua_net_b200.parallel.comm import SymmComm
+
+    for name in ("barrier", "fused_allreduce_sgd", "fused_allreduce_adamw", "fused_clip_reduce_norm", "fused_accum_reduce_norm",
+                 "fused_clip_coef", "fused_clip_apply_sgd", "fused_clip_apply_adamw", "lars_segments", "lars_tensors",
+                 "fused_lars_norm", "fused_lars_trust", "fused_lars_apply", "ema_update", "ema_advance"):
+        want, got = (list(inspect.signature(getattr(c, name)).parameters.values()) for c in (SymmComm, FakeComm))
+        assert [(p.name, p.default) for p in got] == [(p.name, p.default) for p in want], name

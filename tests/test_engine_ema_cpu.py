@@ -1,10 +1,9 @@
 """BnetDDP(ema_decay=...)'s HOST logic on the CPU: the EMA of the master weights against a float64
 torch.optim.swa_utils.AveragedModel (SGD, AdamW and LARS, every 1 and 3, k = 1 and 2, clipped and unclipped), a bucket
 without gradient, set_ema_decay and reset_ema mid-run, the launch order, ema_parameters(), the state dict and its
-cross-loading rules, an engine without EMA, and every rejected argument.  The comm below does the kernels' work in plain
+cross-loading rules, an engine without EMA, and every rejected argument.  FakeComm does the kernels' work in plain
 PyTorch; the kernels are covered on the GPU by tests/test_ema.py."""
 import copy
-import math
 
 import pytest
 import torch
@@ -12,116 +11,7 @@ from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fi
 from engine_fakes import small_model as _model
 from torch.optim.swa_utils import AveragedModel, get_ema_multi_avg_fn
 
-from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_lars_segments, check_lars_tensors
 from bagua_net_b200.parallel.ddp import BnetDDP
-
-
-class EmaComm(FakeComm):
-    """FakeComm plus the staged step, the LARS stages and the two EMA kernels; `log` lists every call in order."""
-
-    def __init__(self):
-        super().__init__()
-        self.log = []
-
-    def fused_allreduce_sgd(self, grad, *a, **k):
-        self.log.append(("update", grad.numel()))
-        super().fused_allreduce_sgd(grad, *a, **k)
-
-    def fused_allreduce_adamw(self, grad, *a, **k):
-        self.log.append(("update", grad.numel()))
-        super().fused_allreduce_adamw(grad, *a, **k)
-
-    def _stage1(self, kind, grad, scratch, partial, add):
-        assert partial.numel() == CLIP_ROW
-        scratch.add_(grad.float()) if add else scratch.copy_(grad.float())
-        partial.zero_()
-        partial[0] = scratch.double().square().sum()
-        grad.zero_()
-        self.launches += 1
-        self.log.append((kind, grad.numel()))
-
-    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("norm", grad, scratch, partial, add=False)
-
-    def fused_accum_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("accum", grad, scratch, partial, add=True)
-
-    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
-        total = torch.tensor(math.sqrt(float(partials.sum())) * grad_scale, dtype=torch.float32)
-        clip[1] = total
-        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
-        self.launches += 1
-        self.log.append(("coef", None))
-
-    def barrier(self, channel=2, stream=None):
-        self.log.append(("barrier", None))
-
-    def fused_clip_apply_sgd(self, param, scratch, clip, master, mom, lr, momentum, weight_decay, grad_scale=None, channel=0,
-                             nblocks=0, stream=None, hp=None):
-        self.log.append(("update", param.numel()))
-        FakeComm.fused_allreduce_sgd(self, scratch * clip[2], param, master, mom, lr, momentum, weight_decay, grad_scale,
-                                     zero_grads=False, hp=hp)
-
-    def fused_clip_apply_adamw(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, channel=0, nblocks=0, stream=None):
-        self.log.append(("update", param.numel()))
-        FakeComm.fused_allreduce_adamw(self, scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, zero_grads=False)
-
-    def lars_segments(self, table, shard_vecs, ntensors):
-        check_lars_segments(table, shard_vecs, ntensors)
-        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
-
-    def lars_tensors(self, table, nslots):
-        check_lars_tensors(table, nslots)
-        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
-
-    def fused_lars_norm(self, master, scratch, segs, slots, dtype, nblocks=0, stream=None):
-        e = 16 // torch.empty((), dtype=dtype).element_size()
-        for vec0, nvec, _, slot0 in segs.tolist():
-            for c in range((nvec + LARS_CHUNK - 1) // LARS_CHUNK):
-                a, b = (vec0 + c * LARS_CHUNK) * e, (vec0 + min(nvec, (c + 1) * LARS_CHUNK)) * e
-                slots[slot0 + c] = torch.stack([master[a:b].double().square().sum(), scratch[a:b].double().square().sum()])
-        self.launches += 1
-        self.log.append(("lars_norm", master.numel()))
-
-    def fused_lars_trust(self, slots, tensors, xchg, clip, hp, scal, trust, channel=0, stream=None):
-        f = lambda v: torch.tensor(float(v), dtype=torch.float32)  # noqa: E731
-        gscale, wd, eta, eps, coef = f(hp[3]), f(hp[2]), f(hp[4]), f(hp[5]), f(clip[2])
-        for j, (slot0, n, excluded, _) in enumerate(tensors.tolist()):
-            w2, g2 = (float(v) for v in slots[slot0:slot0 + n].sum(0)) if n else (0.0, 0.0)
-            wn, gn = f(math.sqrt(w2)), f(math.sqrt(g2) * float(gscale) * float(coef))
-            live = not excluded and wn != 0 and gn != 0
-            t = eta * wn / (gn + wd * wn + eps) if live else torch.tensor(1.0)
-            scal[j, 0], scal[j, 1], trust[j] = gscale * coef * t, wd * t if live else 0.0, t
-        self.launches += 1
-        self.log.append(("lars_trust", None))
-
-    def fused_lars_apply(self, param, scratch, segs, scal, hp, master, mom, channel=0, nblocks=0, stream=None):
-        lr, mu = float(hp[0]), float(hp[1])
-        e = 16 // param.element_size()
-        for vec0, nvec, tensor, _ in segs.tolist():
-            s = slice(vec0 * e, (vec0 + nvec) * e)
-            mom[s].mul_(mu).add_(scratch[s] * scal[tensor, 0] + scal[tensor, 1] * master[s])
-            master[s].sub_(lr * mom[s])
-        param.copy_(master.to(param.dtype))
-        self.launches += 1
-        self.log.append(("update", param.numel()))
-
-    # the EMA kernels: the gate of optim::ema_gate on the block {1 - decay, every, step, n_averaged}, torch.lerp
-    def ema_update(self, master, ema, blk, nblocks=0, stream=None):
-        assert blk.dtype == torch.float32 and blk.numel() == 4 and ema.shape == master.shape
-        w, every, step, n = blk.tolist()
-        if (int(step) + 1) % int(every) == 0:
-            ema.copy_(master if n == 0 else torch.lerp(ema, master, w))
-        self.launches += 1
-        self.log.append(("ema_update", master.numel()))
-
-    def ema_advance(self, blk, stream=None):
-        w, every, step, n = blk.tolist()
-        if (int(step) + 1) % int(every) == 0:
-            blk[3] += 1
-        blk[2] += 1
-        self.launches += 1
-        self.log.append(("ema_advance", None))
 
 
 BATCH = 8
@@ -137,7 +27,7 @@ def _batch(step):
 
 
 def _engine(net, optimizer="sgd", **kw):
-    return BnetDDP(net, optimizer=optimizer, bucket_mb=0.002, comm=EmaComm(), **HYPER[optimizer], **kw)
+    return BnetDDP(net, optimizer=optimizer, bucket_mb=0.002, comm=FakeComm(), **HYPER[optimizer], **kw)
 
 
 def _reference(ref, optimizer):
@@ -269,12 +159,13 @@ def test_launch_order(cpu_engine, kind, k):
     eng = _engine(_model(), optimizer, ema_decay=DECAY, ema_every=2, accumulation_steps=k,
                   max_grad_norm=1.0 if "clipped" in kind else None)
     nb, comm = len(eng.buckets), eng.comm
+    update = "lars_apply" if optimizer == "lars" else "apply" if k > 1 or "clipped" in kind else optimizer
     for step in range(3):
         n0, l0 = len(comm.log), comm.launches
         eng.train_step(*_batch(step))
         kinds = [kind for kind, _ in comm.log[n0:]]
-        last = max(i for i, kd in enumerate(kinds) if kd == "update")
-        assert kinds.count("update") == nb                   # one optimizer step per train_step ...
+        last = max(i for i, kd in enumerate(kinds) if kd == update)
+        assert kinds.count(update) == nb                     # one optimizer step per train_step ...
         assert kinds[last + 1:] == ["ema_update"] * nb + ["ema_advance"]   # ... then the EMA, on every step
         assert [n for kd, n in comm.log[n0:] if kd == "ema_update"] == [b.master.numel() for b in eng.buckets]
         assert comm.launches - l0 == len([kd for kd in kinds if kd != "barrier"])
@@ -364,7 +255,7 @@ def test_engine_without_ema_is_unchanged(cpu_engine):
     for step in range(2):
         n0, l0 = len(eng.comm.log), eng.comm.launches
         eng.train_step(*_batch(step))
-        assert [kind for kind, _ in eng.comm.log[n0:]] == ["update"] * len(eng.buckets)
+        assert [kind for kind, _ in eng.comm.log[n0:]] == ["sgd"] * len(eng.buckets)
         assert eng.comm.launches - l0 == len(eng.buckets)
     state = eng.optimizer_state_dict()
     assert set(state) == SGD_KEYS and all(set(b) == {"master", "momentum"} for b in state["buckets"])

@@ -1,7 +1,7 @@
 """BnetDDP(optimizer="lars")'s HOST logic on the CPU: the segment tables (a pure function, at world 1, 2, 3 and 8), the
 staged step's launch order, the update against a float64 LARC + torch.optim.SGD reference (with and without clipping,
 with accumulation, both memory formats, adopted and accumulated gradients), set_lr mid-run, the state dict, a bucket
-without gradient and every rejected argument.  The comm below does the stages in plain PyTorch with the kernels'
+without gradient and every rejected argument.  FakeComm does the stages in plain PyTorch with the kernels'
 arithmetic; the kernels are covered on the GPU by tests/test_fused_lars.py."""
 import copy
 import math
@@ -11,89 +11,8 @@ import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
 from engine_fakes import small_model as _model
 
-from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_lars_segments, check_lars_tensors
+from bagua_net_b200.parallel.comm import LARS_CHUNK, check_lars_segments, check_lars_tensors
 from bagua_net_b200.parallel.ddp import BnetDDP, lars_segments, plan_buckets
-
-
-class LarsComm(FakeComm):
-    """FakeComm plus the staged step and the three LARS stages; `log` lists every call in order."""
-
-    def __init__(self):
-        super().__init__()
-        self.log = []
-
-    def _stage1(self, kind, grad, scratch, partial, add):
-        assert partial.numel() == CLIP_ROW
-        scratch.add_(grad.float()) if add else scratch.copy_(grad.float())
-        partial.zero_()
-        partial[0] = scratch.double().square().sum()
-        grad.zero_()
-        self.launches += 1
-        self.log.append((kind, grad.numel()))
-
-    def fused_clip_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("norm", grad, scratch, partial, add=False)
-
-    def fused_accum_reduce_norm(self, grad, scratch, partial, channel=0, nblocks=0, stream=None):
-        self._stage1("accum", grad, scratch, partial, add=True)
-
-    def fused_clip_coef(self, partials, xchg, clip, grad_scale=None, channel=0, stream=None):
-        total = torch.tensor(math.sqrt(float(partials.sum())) * grad_scale, dtype=torch.float32)
-        clip[1] = total
-        clip[2] = torch.clamp(clip[0] / (total + 1e-6), max=1.0)
-        self.launches += 1
-        self.log.append(("coef", None))
-
-    def barrier(self, channel=2, stream=None):
-        self.log.append(("barrier", None))
-
-    def lars_segments(self, table, shard_vecs, ntensors):
-        self.nslots_of = getattr(self, "nslots_of", {})
-        t = torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
-        self.nslots_of[id(t)] = check_lars_segments(table, shard_vecs, ntensors)
-        return t
-
-    def lars_tensors(self, table, nslots):
-        check_lars_tensors(table, nslots)
-        return torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
-
-    def fused_lars_norm(self, master, scratch, segs, slots, dtype, nblocks=0, stream=None):
-        e = 16 // torch.empty((), dtype=dtype).element_size()
-        assert slots.shape == (self.nslots_of[id(segs)], 2)
-        for vec0, nvec, _, slot0 in segs.tolist():
-            for c in range((nvec + LARS_CHUNK - 1) // LARS_CHUNK):
-                a, b = (vec0 + c * LARS_CHUNK) * e, (vec0 + min(nvec, (c + 1) * LARS_CHUNK)) * e
-                slots[slot0 + c] = torch.stack([master[a:b].double().square().sum(), scratch[a:b].double().square().sum()])
-        self.launches += 1
-        self.log.append(("lars_norm", master.numel()))
-
-    def fused_lars_trust(self, slots, tensors, xchg, clip, hp, scal, trust, channel=0, stream=None):
-        assert xchg.numel() >= 2 * self.world * tensors.shape[0]
-        f = lambda v: torch.tensor(float(v), dtype=torch.float32)  # noqa: E731
-        gscale, wd, eta, eps, coef = f(hp[3]), f(hp[2]), f(hp[4]), f(hp[5]), f(clip[2])
-        for j, (slot0, n, excluded, _) in enumerate(tensors.tolist()):
-            w2, g2 = (float(v) for v in slots[slot0:slot0 + n].sum(0)) if n else (0.0, 0.0)
-            wn, gn = f(math.sqrt(w2)), f(math.sqrt(g2) * float(gscale) * float(coef))
-            t = torch.tensor(1.0)
-            if not excluded and wn != 0 and gn != 0:
-                t = eta * wn / (gn + wd * wn + eps)
-            scal[j, 0] = gscale * coef * t
-            scal[j, 1] = wd * t if not excluded and wn != 0 and gn != 0 else 0.0
-            trust[j] = t
-        self.launches += 1
-        self.log.append(("lars_trust", tensors.shape[0]))
-
-    def fused_lars_apply(self, param, scratch, segs, scal, hp, master, mom, channel=0, nblocks=0, stream=None):
-        lr, mu = float(hp[0]), float(hp[1])
-        e = 16 // param.element_size()
-        for vec0, nvec, tensor, _ in segs.tolist():
-            s = slice(vec0 * e, (vec0 + nvec) * e)
-            d = scratch[s] * scal[tensor, 0] + scal[tensor, 1] * master[s]
-            mom[s].mul_(mu).add_(d)
-            master[s].sub_(lr * mom[s])
-        param.copy_(master.to(param.dtype))
-        self.launches += 1
-        self.log.append(("lars_apply", param.numel()))
 
 
 # ------------------------------------------------------------------ the segment tables
@@ -187,7 +106,7 @@ def _pair(channels_last=True, model=None, **kw):
     make = model or _model
     ref, net = make(channels_last).double(), make(channels_last)
     opt = torch.optim.SGD(ref.parameters(), lr=LARS["lr"], momentum=LARS["momentum"])
-    eng = BnetDDP(net, optimizer="lars", bucket_mb=0.002, comm=LarsComm(), **LARS, **kw)
+    eng = BnetDDP(net, optimizer="lars", bucket_mb=0.002, comm=FakeComm(), **LARS, **kw)
     return ref, opt, net, eng
 
 
@@ -249,7 +168,7 @@ def test_launch_order(cpu_engine, clipped, k):
 
 def test_other_optimizers_have_no_trust_ratios(cpu_engine):
     for kw in ({}, {"optimizer": "adamw"}):
-        eng = BnetDDP(_model(), bucket_mb=0.002, comm=LarsComm(), **kw)
+        eng = BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), **kw)
         assert eng.last_trust_ratios is None
 
 
@@ -294,7 +213,7 @@ def test_state_dict_round_trip_and_keys(cpu_engine):
         assert all(torch.equal(t1, t2) for t1, t2 in zip(b1.state, b2.state))
     assert torch.equal(resumed._hp, eng._hp)
     for other in ({}, {"optimizer": "adamw"}):
-        plain = BnetDDP(_model(), bucket_mb=0.002, comm=LarsComm(), **other)
+        plain = BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), **other)
         with pytest.raises(ValueError):
             plain.load_optimizer_state_dict(copy.deepcopy(state))
         with pytest.raises(ValueError):
@@ -305,6 +224,6 @@ def test_rejects_bad_arguments(cpu_engine):
     for bad in ({"trust_coefficient": 0.0}, {"trust_coefficient": -1e-3}, {"trust_coefficient": float("nan")},
                 {"eps": -1e-8}, {"eps": float("nan")}, {"amsgrad": True}, {"maximize": True}):
         with pytest.raises(ValueError):
-            BnetDDP(_model(), optimizer="lars", bucket_mb=0.002, comm=LarsComm(), **bad)
+            BnetDDP(_model(), optimizer="lars", bucket_mb=0.002, comm=FakeComm(), **bad)
     with pytest.raises(ValueError):
-        BnetDDP(_model(), optimizer="lamb", bucket_mb=0.002, comm=LarsComm())
+        BnetDDP(_model(), optimizer="lamb", bucket_mb=0.002, comm=FakeComm())

@@ -7,6 +7,7 @@ import subprocess
 import sys
 
 import pytest
+from gpu_jobs import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -21,32 +22,8 @@ def _torch():
 
 
 def _run_worker(name, nproc, extra_env=None, args=(), timeout=300):
-    """One process per GPU, torchrun-style environment, rendezvous on 127.0.0.1."""
-    import socket
-
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = []
-    for r in range(nproc):
-        env = dict(os.environ, RANK=str(r), LOCAL_RANK=str(r), WORLD_SIZE=str(nproc), MASTER_ADDR="127.0.0.1",
-                   MASTER_PORT=str(port), PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-        env.update(extra_env or {})
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "gpu_worker.py"), name, *args],
-                                      env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))
-    outs = []
-    for p in procs:
-        try:
-            o, e = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        outs.append((p.returncode, o, e))
-    for rc, o, e in outs:
-        assert rc == 0, f"worker failed rc={rc}\nstdout:\n{o[-3000:]}\nstderr:\n{e[-3000:]}"
-    return outs
+    """Job `name` of tests/gpu_worker.py as one process per GPU."""
+    return run_ranks(os.path.join(ROOT, "tests", "gpu_worker.py"), (name, *args), nproc, extra_env, timeout)
 
 
 # ------------------------------------------------------------------ transport executor (K1/K4/K5/K7/K8)
@@ -228,30 +205,8 @@ def test_transport_mesh_twoshot_allreduce_2gpu():
 
 
 def _run_script(script, nproc, timeout=300):
-    """A benchmark script of bench/ as one process per GPU (torchrun-style environment); returns rank 0's JSON line."""
-    import socket
-
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = []
-    for r in range(nproc):
-        env = dict(os.environ, RANK=str(r), LOCAL_RANK=str(r), WORLD_SIZE=str(nproc), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                   PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "bench", script)], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.PIPE, text=True))
-    outs = []
-    for p in procs:
-        try:
-            o, e = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        outs.append((p.returncode, o, e))
-    for rc, o, e in outs:
-        assert rc == 0, f"{script} failed rc={rc}\nstdout:\n{o[-2000:]}\nstderr:\n{e[-3000:]}"
+    """A benchmark script of bench/ as one process per GPU; returns rank 0's JSON line and every rank's output."""
+    outs = run_ranks(os.path.join(ROOT, "bench", script), nproc=nproc, timeout=timeout)
     return json.loads([ln for ln in outs[0][1].splitlines() if ln.startswith("{")][-1]), "".join(o + e for _, o, e in outs)
 
 

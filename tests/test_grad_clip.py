@@ -5,11 +5,9 @@ with the one-kernel step at max_norm = inf, the CTA-paired zeroing under stagger
 against torch.optim.AdamW + clip_grad_norm_ in eager and CUDA-graph mode.  The jobs are tests/grad_clip_worker.py; every
 job runs in child processes, one per GPU."""
 import os
-import socket
-import subprocess
-import sys
 
 import pytest
+from gpu_jobs import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -17,39 +15,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORKER = os.path.join(ROOT, "tests", "grad_clip_worker.py")
 
 
-def _run(name, nproc=1, env=None, timeout=600):
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = []
-    for r in range(nproc):
-        e = dict(os.environ, RANK=str(r), LOCAL_RANK=str(r), WORLD_SIZE=str(nproc), MASTER_ADDR="127.0.0.1",
-                 MASTER_PORT=str(port), PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-        e.update(env or {})
-        procs.append(subprocess.Popen([sys.executable, WORKER, name], env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE,
-                                      text=True))
-    outs = []
-    for p in procs:
-        try:
-            o, err = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        outs.append((p.returncode, o, err))
-    for rc, o, err in outs:
-        print(o)
-        assert rc == 0, f"job {name} failed rc={rc}\nstdout:\n{o[-4000:]}\nstderr:\n{err[-4000:]}"
-
-
 @pytest.mark.parametrize("job", ["kernel", "coef", "identity", "staggered", "engine"])
 def test_grad_clip(job):
-    _run(job, timeout=900)
+    run_ranks(WORKER, [job], timeout=900)
 
 
 @pytest.mark.multigpu
 @pytest.mark.parametrize("env", [{}, {"BNET_FUSED_NVLS": "0"}], ids=["auto", "p2p"])
 @pytest.mark.parametrize("job", ["kernel", "coef", "identity", "staggered", "engine"])
 def test_grad_clip_2gpu(job, env):
-    _run(job, nproc=2, env=env, timeout=900)
+    run_ranks(WORKER, [job], nproc=2, env=env, timeout=900)
