@@ -91,6 +91,11 @@ $(BUILD)/tests/optim_emu_test: csrc/tests/optim_emu_test.cc csrc/cuda/optim_body
 	@mkdir -p $(dir $@)
 	$(CXX) $(EMU_FLAGS) $< -o $@
 
+# the parameter-group lookup of the fused optimizer kernels against a brute-force map
+$(BUILD)/tests/group_lookup_test: csrc/tests/group_lookup_test.cc csrc/cuda/optim_body.cuh
+	@mkdir -p $(dir $@)
+	$(CXX) $(EMU_FLAGS) $< -o $@
+
 # the same emulation tests under Address/UB sanitizers: an out-of-bounds or misaligned access of a kernel body
 # is caught here, on the CPU, instead of poisoning a CUDA context
 emu-asan: csrc/tests/nn_emu_test.cc csrc/tests/exec_emu_test.cc csrc/tests/tc_emu_test.cc csrc/tests/optim_emu_test.cc csrc/cuda/nn_body.cuh csrc/cuda/exec_body.cuh csrc/cuda/tc_body.cuh csrc/cuda/optim_body.cuh
@@ -104,13 +109,15 @@ emu-asan: csrc/tests/nn_emu_test.cc csrc/tests/exec_emu_test.cc csrc/tests/tc_em
 	$(BUILD)/asan/tests/tc_emu_test
 	$(BUILD)/asan/tests/optim_emu_test
 
-test: $(TEST_BINS) $(BUILD)/tests/nn_emu_test $(BUILD)/tests/exec_emu_test $(BUILD)/tests/tc_emu_test $(BUILD)/tests/optim_emu_test
+test: $(TEST_BINS) $(BUILD)/tests/nn_emu_test $(BUILD)/tests/exec_emu_test $(BUILD)/tests/tc_emu_test $(BUILD)/tests/optim_emu_test \
+      $(BUILD)/tests/group_lookup_test
 	$(BUILD)/tests/unit_tests $(PLUGIN_SO)
 	$(BUILD)/tests/loopback_test $(PLUGIN_SO)
 	$(BUILD)/tests/nn_emu_test
 	$(BUILD)/tests/exec_emu_test
 	$(BUILD)/tests/tc_emu_test
 	$(BUILD)/tests/optim_emu_test
+	$(BUILD)/tests/group_lookup_test
 
 BENCH_BINS := $(BUILD)/bench/all_reduce_perf
 NCCL_HOME ?= $(shell python -c "import nvidia.nccl, os; print(os.path.dirname(nvidia.nccl.__file__))" 2>/dev/null)

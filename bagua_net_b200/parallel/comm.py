@@ -27,6 +27,7 @@ ALGOS = {"auto": 0, "nvls": 1, "p2p": 2, "oneshot": 3, "ll": 0}
 BLOB = 128
 CLIP_ROW = 304          # doubles per bucket in the clipped step's partial rows (BNET_COLL_CLIP_ROW)
 LARS_CHUNK = 4096       # vectors per norm slot of the LARS norm pass (BNET_LARS_CHUNK)
+GROUPS_MAX = 64         # parameter groups of one engine, its default group included (BNET_GROUPS_MAX)
 
 
 def check_lars_segments(table, shard_vecs: int, ntensors: int) -> int:
@@ -52,6 +53,28 @@ def check_lars_segments(table, shard_vecs: int, ntensors: int) -> int:
     if pos != shard_vecs:
         raise ValueError(f"LARS segments cover {pos} of the shard's {shard_vecs} vectors")
     return slots
+
+
+def check_group_segments(table, shard_vecs: int, ngroups: int) -> None:
+    """Validate a parameter-group segment table (rows {vec0, nvec, group, reserved}, see include/bnet/bnet_coll.h) for a
+    shard of `shard_vecs` 16-byte vectors before it goes to the device, where the kernels trust it: sorted, covering the
+    shard exactly once, group indices below `ngroups` (1..GROUPS_MAX).  Raises ValueError."""
+    rows = [tuple(int(v) for v in r) for r in torch.as_tensor(table).reshape(-1, 4).tolist()]
+    if not rows:
+        raise ValueError("group segment table is empty")
+    if not 0 < shard_vecs < 2 ** 31:
+        raise ValueError(f"group shard of {shard_vecs} vectors is out of range")
+    if not 1 <= ngroups <= GROUPS_MAX:
+        raise ValueError(f"{ngroups} parameter groups: the kernels take 1..{GROUPS_MAX}")
+    pos = 0
+    for k, (vec0, nvec, group, _) in enumerate(rows):
+        if vec0 != pos or nvec < 1 or pos + nvec > shard_vecs:
+            raise ValueError(f"group segment {k} ({vec0}, {nvec}) does not continue the cover of the shard at vector {pos}")
+        if not 0 <= group < ngroups:
+            raise ValueError(f"group segment {k} names group {group} of {ngroups}")
+        pos += nvec
+    if pos != shard_vecs:
+        raise ValueError(f"group segments cover {pos} of the shard's {shard_vecs} vectors")
 
 
 def check_lars_tensors(table, nslots: int) -> None:
@@ -124,6 +147,10 @@ def _declare(lib):
     lib.bnet_fused_lars_norm.argtypes = [vp, sz, i, vp, vp, vp, i, vp, i, i, vp]
     lib.bnet_fused_lars_trust.argtypes = [vp, vp, vp, i, sz, vp, vp, vp, vp, i, vp]
     lib.bnet_fused_lars_apply.argtypes = [vp, sz, sz, i, vp, vp, i, vp, vp, vp, vp, i, i, vp]
+    lib.bnet_fused_allreduce_sgd_groups.argtypes = [vp, sz, sz, sz, i, vp, vp, i, vp, i, vp, vp, i, i, i, vp]
+    lib.bnet_fused_allreduce_adamw_groups.argtypes = [vp, sz, sz, sz, i, vp, vp, i, vp, i, vp, vp, vp, i, i, i, vp]
+    lib.bnet_fused_clip_apply_sgd_groups.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, i, vp, i, vp, vp, i, i, vp]
+    lib.bnet_fused_clip_apply_adamw_groups.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, i, vp, i, vp, vp, vp, i, i, vp]
     lib.bnet_ema_update.argtypes = [vp, sz, vp, vp, vp, i, vp]
     lib.bnet_ema_advance.argtypes = [vp, vp, vp]
     lib.bnet_pack_cast.argtypes = [vp, i, vp, i, i, C.c_float, C.c_uint64, vp]
@@ -177,6 +204,7 @@ class SymmComm:
         self._heap = torch.as_tensor(_CudaView(self.heap_ptr, self.heap_bytes, self), device=f"cuda:{self.device}")
         self._bump = 0
         self._lars_tables = {}     # device address of every validated LARS table -> (kind, rows, shard vectors or slots)
+        self._group_tables = {}    # device address of every validated group segment table -> (rows, shard vectors, groups)
         # area of the barrier-free small-message all-reduce ("LL": the flag travels inside every 8-byte word)
         self.ll_words = int(os.environ.get("BNET_LL_WORDS", "8192"))          # 32 KiB of payload per rank and call
         area = int(self.lib.bnet_allreduce_ll_area_bytes(self.world, self.ll_words))
@@ -464,6 +492,58 @@ class SymmComm:
             C.c_void_p(segs.data_ptr()), segs.shape[0], C.c_void_p(scal.data_ptr()), C.c_void_p(hp.data_ptr()),
             C.c_void_p(master.data_ptr()), C.c_void_p(mom.data_ptr()), channel, nblocks, self._stream(stream)), "fused_lars_apply")
         self.launches += n
+
+    # ------------------------------------------------------------------ parameter groups: per-group lr and weight decay
+    def group_segments(self, table, shard_vecs: int, ngroups: int) -> torch.Tensor:
+        """Validate a bucket's parameter-group segment table on the host (``check_group_segments``) and upload it: the
+        grouped kernels accept only tables that went through here.  Returns the [nseg, 4] int32 device tensor."""
+        check_group_segments(table, shard_vecs, ngroups)
+        t = torch.as_tensor(table, dtype=torch.int32).reshape(-1, 4).to(f"cuda:{self.device}").contiguous()
+        self._group_tables[t.data_ptr()] = (t, shard_vecs, ngroups)
+        return t
+
+    def _grouped_args(self, param, hp, hp_words, groups, segs):
+        """The checks of the grouped entry points: ``hp`` the optimizer's device block, ``groups`` the [G, 4] fp32 group
+        table (at least as many rows as ``segs`` was validated for), ``segs`` from ``group_segments`` for this shard."""
+        rec = self._group_tables.get(segs.data_ptr())
+        if rec is None or rec[0] is not segs or rec[1] != param.numel() * param.element_size() // 16 // self.world:
+            raise ValueError("group segment table was not validated for this shard: upload it with SymmComm.group_segments")
+        assert hp.is_cuda and hp.dtype == torch.float32 and hp.numel() >= hp_words and hp.is_contiguous()
+        assert groups.is_cuda and groups.dtype == torch.float32 and groups.is_contiguous() and groups.dim() == 2
+        assert groups.shape[1] == 4 and rec[2] <= groups.shape[0] <= GROUPS_MAX
+        return (C.c_void_p(hp.data_ptr()), C.c_void_p(groups.data_ptr()), groups.shape[0], C.c_void_p(segs.data_ptr()),
+                segs.shape[0])
+
+    def fused_allreduce_sgd_groups(self, grad: torch.Tensor, param: torch.Tensor, master: torch.Tensor, mom: torch.Tensor,
+                                   hp: torch.Tensor, groups: torch.Tensor, segs: torch.Tensor, zero_grads: bool = True,
+                                   channel: int = 0, nblocks: int = 0, stream=None):
+        """``fused_allreduce_sgd`` with every tensor's lr and weight decay from its group's row {lr, weight_decay,
+        reserved, reserved} of ``groups``, found through ``segs``; momentum and gradient scale from the 4-float ``hp``."""
+        self._fused_step("fused_allreduce_sgd_groups", grad, param, (master, mom), self._grouped_args(param, hp, 4, groups, segs),
+                         None, 0, zero_grads, channel, nblocks, stream)
+
+    def fused_allreduce_adamw_groups(self, grad: torch.Tensor, param: torch.Tensor, master: torch.Tensor,
+                                     exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, hp: torch.Tensor, groups: torch.Tensor,
+                                     segs: torch.Tensor, zero_grads: bool = True, channel: int = 0, nblocks: int = 0,
+                                     stream=None):
+        """``fused_allreduce_adamw`` with every tensor's lr and weight decay from its group's row of ``groups``."""
+        self._fused_step("fused_allreduce_adamw_groups", grad, param, (master, exp_avg, exp_avg_sq),
+                         self._grouped_args(param, hp, 8, groups, segs), None, 0, zero_grads, channel, nblocks, stream)
+
+    def fused_clip_apply_sgd_groups(self, param: torch.Tensor, scratch: torch.Tensor, clip: torch.Tensor, master: torch.Tensor,
+                                    mom: torch.Tensor, hp: torch.Tensor, groups: torch.Tensor, segs: torch.Tensor,
+                                    channel: int = 0, nblocks: int = 0, stream=None):
+        """Stage 3, per bucket: ``fused_clip_apply_sgd`` with the per-group lr and weight decay of ``groups``."""
+        self._clip_apply("fused_clip_apply_sgd_groups", param, scratch, clip, (master, mom),
+                         self._grouped_args(param, hp, 4, groups, segs), None, 0, channel, nblocks, stream)
+
+    def fused_clip_apply_adamw_groups(self, param: torch.Tensor, scratch: torch.Tensor, clip: torch.Tensor,
+                                      master: torch.Tensor, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, hp: torch.Tensor,
+                                      groups: torch.Tensor, segs: torch.Tensor, channel: int = 0, nblocks: int = 0,
+                                      stream=None):
+        """Stage 3, per bucket: ``fused_clip_apply_adamw`` with the per-group lr and weight decay of ``groups``."""
+        self._clip_apply("fused_clip_apply_adamw_groups", param, scratch, clip, (master, exp_avg, exp_avg_sq),
+                         self._grouped_args(param, hp, 8, groups, segs), None, 0, channel, nblocks, stream)
 
     # ------------------------------------------------------------------ exponential moving average of the master weights
     def ema_update(self, master: torch.Tensor, ema: torch.Tensor, blk: torch.Tensor, nblocks: int = 0, stream=None):

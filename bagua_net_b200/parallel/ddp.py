@@ -16,11 +16,12 @@ NVSwitch box:
 from __future__ import annotations
 
 import contextlib
+import math
 
 import torch
 import torch.distributed as dist
 
-from .comm import LARS_CHUNK, SymmComm
+from .comm import GROUPS_MAX, LARS_CHUNK, SymmComm
 
 
 def plan_buckets(numels, element_size: int, world: int, bucket_mb: float):
@@ -169,6 +170,83 @@ def lars_segments(members, numels, start: int, numel: int, element_size: int, wo
     return table
 
 
+def group_segments(members, numels, group_of, start: int, numel: int, element_size: int, world: int, rank: int):
+    """The parameter-group segment table of one bucket on one rank: rows [vec0, nvec, group, 0] (include/bnet/bnet_coll.h),
+    the LARS segments of ``lars_segments`` with every tensor mapped to its group (``group_of[parameter index]``) and
+    adjacent rows of the same group merged.  Padding goes with the segment it joins there."""
+    rows = []
+    for vec0, nvec, pi, _ in lars_segments(members, numels, start, numel, element_size, world, rank):
+        if rows and rows[-1][2] == group_of[pi]:
+            rows[-1][1] += nvec
+        else:
+            rows.append([vec0, nvec, group_of[pi], 0])
+    return rows
+
+
+def no_weight_decay_groups(module: torch.nn.Module, names=()) -> list:
+    """The usual param group without weight decay: ``[{"params": [...], "weight_decay": 0.0}]`` with every trainable
+    parameter of ``module`` that has ``p.dim() <= 1`` (biases, normalisation weights) or whose name (as in
+    ``module.named_parameters()``) is in ``names``.  Pass it, with any groups of your own, as ``BnetDDP(param_groups=...)``."""
+    names = set(names)
+    named = dict(module.named_parameters())
+    unknown = names - set(named)
+    if unknown:
+        raise ValueError(f"no_weight_decay_groups: {sorted(unknown)} are not parameters of the module")
+    return [{"params": [p for n, p in named.items() if p.requires_grad and (p.dim() <= 1 or n in names)], "weight_decay": 0.0}]
+
+
+def _check_group_value(key: str, v) -> float:
+    try:
+        v = float(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"param group {key!r} must be a number (got {v!r})") from None
+    if not 0.0 <= v < math.inf:           # (False for NaN as well)
+        raise ValueError(f"param group {key!r} must be finite and >= 0 (got {v})")
+    return v
+
+
+def _parse_param_groups(param_groups, params):
+    """(group of every trainable parameter, lr_scale per group, weight_decay per group or None) from the user's list of
+    dicts; the parameters no group lists form the default group, last.  Raises ValueError."""
+    if isinstance(param_groups, dict) or not isinstance(param_groups, (list, tuple)):
+        raise ValueError("param_groups must be a list of dicts, as torch.optim takes them")
+    index = {id(p): i for i, p in enumerate(params)}
+    group_of = [None] * len(params)
+    scales, wds = [], []
+    for k, g in enumerate(param_groups):
+        if not isinstance(g, dict):
+            raise ValueError(f"param group {k} is not a dict")
+        extra = set(g) - {"params", "lr_scale", "weight_decay"}
+        if "lr" in extra:
+            raise ValueError(f"param group {k} sets 'lr': give a multiplier of the engine's lr as 'lr_scale' instead, so "
+                             "that set_lr and a schedule move every group")
+        if extra:
+            raise ValueError(f"param group {k} has unknown keys {sorted(extra)}: a group takes 'params', 'lr_scale' and "
+                             "'weight_decay' (the other hyper-parameters are the engine's)")
+        if "params" not in g:
+            raise ValueError(f"param group {k} has no 'params'")
+        ps = g["params"]
+        ps = [ps] if isinstance(ps, torch.Tensor) else list(ps)
+        if not ps:
+            raise ValueError(f"param group {k} has no parameters")
+        for p in ps:
+            i = index.get(id(p))
+            if i is None or params[i] is not p:
+                raise ValueError(f"param group {k} lists a tensor that is not a trainable parameter of the module")
+            if group_of[i] is not None:
+                raise ValueError(f"a parameter is in param groups {group_of[i]} and {k}")
+            group_of[i] = k
+        scales.append(_check_group_value("lr_scale", g.get("lr_scale", 1.0)))
+        wds.append(_check_group_value("weight_decay", g["weight_decay"]) if "weight_decay" in g else None)
+    if any(g is None for g in group_of):
+        group_of = [len(scales) if g is None else g for g in group_of]
+        scales.append(1.0)
+        wds.append(None)
+    if len(scales) > GROUPS_MAX:
+        raise ValueError(f"{len(scales)} param groups (the default group included): the kernels take at most {GROUPS_MAX}")
+    return group_of, scales, wds
+
+
 def _check_max_norm(v) -> float:
     v = float(v)
     if not v > 0.0:                       # (False for NaN as well)
@@ -187,7 +265,8 @@ def _check_ema_decay(v) -> float:
 
 
 class _Bucket:
-    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state", "scratch", "partial", "launched", "ema")
+    __slots__ = ("params", "start", "numel", "ready", "grad", "param", "state", "scratch", "partial", "launched", "ema",
+                 "gsegs")
 
     def __init__(self):
         self.params = []
@@ -198,6 +277,7 @@ class _Bucket:
         self.partial = None          # staged step: the bucket's row of per-CTA sums of squares
         self.launched = False        # staged step: stage 1 ran for this bucket in the current step (the scratch holds data)
         self.ema = None              # EMA of the master shard (fp32, same layout), kept apart from the optimizer's state
+        self.gsegs = None            # parameter groups: the validated group segment table of this rank's shard
 
     @property
     def master(self) -> torch.Tensor:
@@ -240,6 +320,15 @@ class BnetDDP(torch.nn.Module):
     decides on its own which steps update.  Buffers (BatchNorm statistics) are not averaged.  Evaluate or save the
     averaged model inside ``with engine.ema_parameters():``; ``set_ema_decay`` and ``reset_ema`` change it between steps.
     ``None`` keeps no EMA.
+
+    param_groups: per-group learning rate and weight decay for ``"sgd"`` and ``"adamw"``, as torch.optim's param groups:
+    a list of dicts with ``"params"`` (trainable parameters of ``module``), optionally ``"lr_scale"`` (>= 0, default 1:
+    the group's lr is ``lr * lr_scale``) and ``"weight_decay"`` (>= 0, fixed for the group; without it the group follows
+    the engine's ``weight_decay``).  Parameters no group lists form a default group, last.  At most 64 groups, the default
+    one included.  ``no_weight_decay_groups(module)`` gives the usual group of biases and normalisation weights without
+    decay.  Groups change neither the buckets nor the state layout; ``set_lr`` moves every group's lr through its scale
+    and ``set_param_group`` changes one group, both without re-capturing a CUDA graph.  ``None`` keeps one lr and one
+    weight decay for every parameter.
     """
 
     def __init__(self, module: torch.nn.Module, lr: float = 0.01, momentum: float | None = None, weight_decay: float = 0.0,
@@ -247,7 +336,7 @@ class BnetDDP(torch.nn.Module):
                  nblocks: int = 0, group=None, optimizer: str = "sgd", betas: tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, amsgrad: bool = False, maximize: bool = False, max_grad_norm: float | None = None,
                  accumulation_steps: int = 1, trust_coefficient: float = 0.001, ema_decay: float | None = None,
-                 ema_every: int = 1):
+                 ema_every: int = 1, param_groups: list | None = None):
         super().__init__()
         if ema_decay is not None:
             ema_decay = _check_ema_decay(ema_decay)
@@ -288,6 +377,12 @@ class BnetDDP(torch.nn.Module):
             raise ValueError("BnetDDP expects a single parameter dtype (bf16 or fp32)")
         if dtype not in (torch.bfloat16, torch.float32):
             raise ValueError(f"unsupported parameter dtype {dtype}")
+        self._groups = None
+        if param_groups is not None:
+            if optimizer == "lars":
+                raise ValueError("param_groups are offered for 'sgd' and 'adamw'; LARS excludes p.dim() <= 1 tensors itself")
+            self._group_of, self._group_scale, self._group_wd = _parse_param_groups(param_groups, params)
+            self._params = params
         self.dtype = dtype
         es = params[0].element_size()
         world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -403,6 +498,8 @@ class BnetDDP(torch.nn.Module):
         self.max_grad_norm = max_grad_norm
         if optimizer == "lars":
             self._lars_setup(params, plan, es, dev)
+        if param_groups is not None:
+            self._groups_setup(params, plan, es, dev)
         # the EMA of the master shards, starting as their copy (AveragedModel deep-copies the model), and its device block
         self.ema_decay, self.ema_every, self._ema, self._in_ema = ema_decay, ema_every, None, False
         if ema_decay is not None:
@@ -442,6 +539,10 @@ class BnetDDP(torch.nn.Module):
             stage1 = self.comm.fused_accum_reduce_norm if b.launched else self.comm.fused_clip_reduce_norm
             stage1(b.grad, b.scratch, b.partial, channel=0, nblocks=self.nblocks, stream=self.comm_stream)
             b.launched = True
+        elif self._groups is not None:
+            step = self.comm.fused_allreduce_adamw_groups if self.optimizer == "adamw" else self.comm.fused_allreduce_sgd_groups
+            step(b.grad, b.param, *b.state, self._hp, self._groups, b.gsegs, zero_grads=True, channel=0, nblocks=self.nblocks,
+                 stream=self.comm_stream)
         elif self.optimizer == "adamw":
             self.comm.fused_allreduce_adamw(b.grad, b.param, *b.state, self._hp, zero_grads=True, channel=0,
                                             nblocks=self.nblocks, stream=self.comm_stream)
@@ -512,7 +613,11 @@ class BnetDDP(torch.nn.Module):
         for b in self.buckets:
             if not b.launched:
                 continue
-            if self.optimizer == "adamw":
+            if self._groups is not None:
+                apply = self.comm.fused_clip_apply_adamw_groups if self.optimizer == "adamw" else self.comm.fused_clip_apply_sgd_groups
+                apply(b.param, b.scratch, coef, *b.state, self._hp, self._groups, b.gsegs, channel=0, nblocks=self.nblocks,
+                      stream=self.comm_stream)
+            elif self.optimizer == "adamw":
                 self.comm.fused_clip_apply_adamw(b.param, b.scratch, coef, *b.state, self._hp, channel=0,
                                                  nblocks=self.nblocks, stream=self.comm_stream)
             else:
@@ -520,6 +625,59 @@ class BnetDDP(torch.nn.Module):
                                                self.weight_decay, self._grad_scale, channel=0, nblocks=self.nblocks,
                                                stream=self.comm_stream, hp=self._hp)
             b.launched = False
+
+    # ------------------------------------------------------------------ parameter groups
+    def _groups_setup(self, params, plan, es, dev):
+        """Per bucket the validated group segment table of this rank's shard; the device group table; for SGD the
+        4-float block the grouped kernels read momentum and gradient scale from (their lr and weight decay are unused)."""
+        numels = [p.numel() for p in params]
+        G = len(self._group_scale)
+        for b, (start, numel, members) in zip(self.buckets, plan):
+            table = group_segments(members, numels, self._group_of, start, numel, es, self.comm.world, self.comm.rank)
+            b.gsegs = self.comm.group_segments(table, numel // self.comm.world * es // 16, G)
+        self._groups = torch.zeros(G, 4, dtype=torch.float32, device=dev)
+        if self.optimizer == "sgd":
+            self._hp = torch.tensor([self.lr, self.momentum, self.weight_decay, self._grad_scale], dtype=torch.float32,
+                                    device=dev)
+        self._write_groups()
+
+    def _write_groups(self) -> None:
+        """The device group table {lr, weight_decay, 0, 0} per group from the host values: lr = engine lr * lr_scale in
+        double, rounded once to fp32 (as torch rounds a Python-float group lr)."""
+        if self._groups is None:
+            return
+        rows = [[self.lr * s, self.weight_decay if wd is None else wd, 0.0, 0.0] for s, wd in zip(self._group_scale, self._group_wd)]
+        self._groups.copy_(torch.tensor(rows, dtype=torch.float64).to(torch.float32))
+
+    def _require_groups(self, what: str) -> None:
+        if self._groups is None:
+            raise ValueError(f"cannot {what}: the engine has no param groups (build it with param_groups=...)")
+
+    @property
+    def param_groups(self) -> list | None:
+        """Copies of the parameter groups, default group last: ``{"params", "lr_scale", "weight_decay", "lr"}`` with the
+        effective values (a group that follows the engine shows the engine's weight decay).  Changing them changes
+        nothing; use ``set_lr`` and ``set_param_group``.  ``None`` without groups."""
+        if self._groups is None:
+            return None
+        return [{"params": [p for p, g in zip(self._params, self._group_of) if g == k], "lr_scale": s,
+                 "weight_decay": self.weight_decay if wd is None else wd, "lr": self.lr * s}
+                for k, (s, wd) in enumerate(zip(self._group_scale, self._group_wd))]
+
+    def set_param_group(self, i: int, lr_scale: float | None = None, weight_decay: float | None = None) -> None:
+        """Change group ``i``'s lr_scale and/or weight decay (a fixed weight decay from then on) between steps.  Only the
+        device group table is rewritten, so a captured CUDA graph follows without being re-captured."""
+        self._require_groups("set a param group")
+        if isinstance(i, bool) or not isinstance(i, int) or not 0 <= i < len(self._group_scale):
+            raise ValueError(f"param group {i!r} does not exist (the engine has {len(self._group_scale)})")
+        s = self._group_scale[i] if lr_scale is None else _check_group_value("lr_scale", lr_scale)
+        wd = self._group_wd[i] if weight_decay is None else _check_group_value("weight_decay", weight_decay)
+        self._group_scale[i], self._group_wd[i] = s, wd
+        self._write_groups()
+
+    def _groups_state(self) -> list:
+        return [{"params": [j for j, g in enumerate(self._group_of) if g == k], "lr_scale": s, "weight_decay": wd}
+                for k, (s, wd) in enumerate(zip(self._group_scale, self._group_wd))]
 
     # ------------------------------------------------------------------ LARS
     def _lars_setup(self, params, plan, es, dev):
@@ -776,6 +934,8 @@ class BnetDDP(torch.nn.Module):
                     "trust_coefficient": self.trust_coefficient, "eps": self.eps}
         else:
             head = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
+        if self._groups is not None:
+            head["param_groups"] = self._groups_state()
         names = _STATE_NAMES[self.optimizer]
         buckets = [{k: t.detach().cpu() for k, t in zip(names, b.state)} for b in self.buckets]
         if self._ema is not None:
@@ -799,6 +959,15 @@ class BnetDDP(torch.nn.Module):
         for b, s in zip(self.buckets, state["buckets"]):
             if s["master"].shape != b.master.shape or (has_ema and s["ema"].shape != b.master.shape):
                 raise ValueError("optimizer state shard does not match this bucket")
+        groups = state.get("param_groups")
+        if (groups is None) != (self._groups is None):
+            raise ValueError("the optimizer state and this engine disagree on param groups: one has them, the other not")
+        if groups is not None:
+            if [list(g["params"]) for g in groups] != [g["params"] for g in self._groups_state()]:
+                raise ValueError("the optimizer state's param groups hold other parameters than this engine's")
+            scales = [_check_group_value("lr_scale", g["lr_scale"]) for g in groups]
+            wds = [None if g["weight_decay"] is None else _check_group_value("weight_decay", g["weight_decay"]) for g in groups]
+            self._group_scale, self._group_wd = scales, wds
         for b, s in zip(self.buckets, state["buckets"]):
             for k, t in zip(_STATE_NAMES[self.optimizer], b.state):
                 t.copy_(s[k])
@@ -814,6 +983,7 @@ class BnetDDP(torch.nn.Module):
             self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
             self.betas = tuple(state["betas"])
             self._hp.copy_(torch.tensor(self._adamw_hp(state["step"]), dtype=torch.float32))
+            self._write_groups()
             return
         if self.optimizer == "lars":
             self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
@@ -857,6 +1027,7 @@ class BnetDDP(torch.nn.Module):
                 self.weight_decay = float(weight_decay)
             # everything but the step count, which the captured steps advance on the device
             self._hp[:self._HP_STEP].copy_(torch.tensor(self._adamw_hp(0)[:self._HP_STEP], dtype=torch.float32))
+            self._write_groups()
             return
         self.lr = float(lr)
         if momentum is not None:
@@ -872,6 +1043,7 @@ class BnetDDP(torch.nn.Module):
             self._graph = None
         else:
             self._hp.copy_(torch.tensor(vals, dtype=torch.float32), non_blocking=False)
+        self._write_groups()                   # (every group's lr follows through its scale)
 
     def set_max_grad_norm(self, max_norm: float) -> None:
         """Change the clipping threshold of an engine built with ``max_grad_norm``.  The norm kernel reads it from

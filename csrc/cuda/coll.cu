@@ -536,6 +536,55 @@ struct LarsOpt {
   float lr, mu;
 };
 
+// Parameter groups: the step of SgdOpt / AdamWOpt with every vector's group's scalars.  `at(v)` finds shard vector v's
+// group in the sorted segment table with a per-thread cursor (optim::group_seg_advance; v only increases within a
+// thread) and returns the ungrouped policy with that group's values, from shared memory.  The cursor starts at the
+// thread's first vector.
+struct GroupSegs {
+  const int* seg;   // BnetGroupSeg rows, 4 ints each
+  int nseg;
+  mutable int cur;
+  __device__ __forceinline__ GroupSegs(const int4* s, int n)
+      : seg(reinterpret_cast<const int*>(s)), nseg(n), cur(optim::group_seg_find(seg, n, (int)(blockIdx.x * kThreads + threadIdx.x))) {}
+  __device__ __forceinline__ int group(size_t v) const {
+    cur = optim::group_seg_advance(seg, nseg, cur, (int)v);
+    return __ldg(seg + 4 * cur + 2);
+  }
+};
+// SGD: {lr, weight decay} per group in shared memory; momentum and gradient scale are the step's.  U vectors per batch.
+template <int U>
+struct SgdGroupsOpt {
+  static constexpr int kStates = 2;   // master, momentum
+  static constexpr int kU = U;
+  float mu, gscale;
+  const float2* grp;
+  GroupSegs segs;
+  __device__ __forceinline__ SgdOpt at(size_t v) const {
+    const float2 s = grp[segs.group(v)];
+    return SgdOpt{s.x, mu, s.y, gscale};
+  }
+};
+// AdamW: every group's coefficients, computed once per CTA into shared memory.  Only decay and step_size depend on the
+// group's lr and weight decay; the others are the same in every row and stay in registers (`c`, group 0's row), so a
+// vector reads two floats.  (Copying a whole row per vector spills the bf16 variants.)  One vector per batch, as AdamWOpt.
+struct AdamWGroupsOpt {
+  static constexpr int kStates = 3;   // master, exp_avg, exp_avg_sq
+  static constexpr int kU = 1;
+  optim::AdamWCoef c;
+  const optim::AdamWCoef* coef;
+  GroupSegs segs;
+  __device__ __forceinline__ AdamWOpt at(size_t v) const {
+    const optim::AdamWCoef& r = coef[segs.group(v)];
+    AdamWOpt o{c};
+    o.c.decay = r.decay;
+    o.c.step_size = r.step_size;
+    return o;
+  }
+};
+template <class Opt> constexpr bool kGroupedOpt = false;
+template <int U> constexpr bool kGroupedOpt<SgdGroupsOpt<U>> = true;
+template <> constexpr bool kGroupedOpt<AdamWGroupsOpt> = true;
+
 // One batch = U 16-byte gradient vectors per thread.  All loads of the batch (in-switch reductions / peer loads or the
 // fp32 scratch, the fp32 state) are issued before any dependent math so that U*(1 + S*E/4) requests per thread are in
 // flight: the kernel is latency*bandwidth bound (NVLink round trip ~3 us, HBM), not ALU bound.
@@ -596,6 +645,10 @@ __device__ __forceinline__ void fused_batch(const CollDev& d, const G& src, size
     if constexpr (kLars) {
       // per-element sgd_update with the vector's scalars: g already carries its gradient scale
       const SgdOpt o{opt.lr, opt.mu, sc.y, 1.0f};
+#pragma unroll
+      for (int k = 0; k < E; k++) o.update(g[k], st, k);
+    } else if constexpr (kGroupedOpt<Opt>) {
+      const auto o = opt.at(i + u * stride);
 #pragma unroll
       for (int k = 0; k < E; k++) o.update(g[k], st, k);
     } else {
@@ -811,6 +864,91 @@ __global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_adamw_kernel(Coll
   float* const state[3] = {master, exp_avg, exp_avg_sq};
   fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec, AdamWOpt{optim::adamw_coef(hp)}, state, 0,
                        chan);
+}
+
+// ------------------------------------------------------------------ parameter groups: per-group lr and weight decay
+// The one-kernel steps (HeapGrad) and the staged step's apply stage (ScratchGrad) of SGD and AdamW with each vector's
+// group's lr and weight decay from the group table (rows of optim::kGroupWords floats), found through the bucket's
+// segment table.  Everything else -- barriers, gradient zeroing, parameter broadcast -- is fused_step's, unchanged.
+//
+// SGD: the first ngroups threads copy {lr, weight decay} of every group into shared memory; momentum and gradient
+// scale come from the 4-float SGD block, whose lr and weight decay are not read.
+__device__ __forceinline__ void sgd_groups_load(const float4* __restrict__ groups, int ngroups, float2* grp) {
+  if ((int)threadIdx.x < ngroups) {
+    const float4 r = groups[threadIdx.x];
+    grp[threadIdx.x] = make_float2(r.x, r.y);
+  }
+  __syncthreads();
+}
+// AdamW: the first ngroups threads compute every group's coefficients with the unchanged optim::adamw_coef on a copy of
+// the 8-float block with the group's lr and weight decay, so a group's elements get the bits of the ungrouped kernel
+// run with those two values.  Before the opening rank barrier, where the wait for the peers hides it.
+__device__ __forceinline__ void adamw_groups_coef(const float* __restrict__ hp, const float4* __restrict__ groups, int ngroups,
+                                                  optim::AdamWCoef* coef) {
+  if ((int)threadIdx.x < ngroups) {
+    float h[optim::kHpWords];
+#pragma unroll
+    for (int k = 0; k < optim::kHpWords; k++) h[k] = hp[k];
+    const float4 r = groups[threadIdx.x];
+    h[optim::kHpLr] = r.x;
+    h[optim::kHpWeightDecay] = r.y;
+    coef[threadIdx.x] = optim::adamw_coef(h);
+  }
+  __syncthreads();
+}
+// Vectors per batch of the grouped SGD kernels: two, as SgdOpt, except in the bf16 apply stage, where the lookup on top
+// of two vectors' scratch and state loads spills at the 64-register cap of two 512-thread CTAs per SM (as LarsOpt).
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_fused_sgd_groups_kernel(CollDev d, size_t goff, size_t poff, size_t nvec,
+                                                                        const float* __restrict__ hp, const float4* __restrict__ groups,
+                                                                        int ngroups, const int4* __restrict__ seg, int nseg,
+                                                                        float* __restrict__ master, float* __restrict__ mom,
+                                                                        int zero_grads, int chan) {
+  __shared__ float2 grp[BNET_GROUPS_MAX];
+  sgd_groups_load(groups, ngroups, grp);
+  float* const state[2] = {master, mom};
+  fused_step<DT, MODE>(d, HeapGrad{goff}, poff, nvec, SgdGroupsOpt<2>{hp[1], hp[3], grp, GroupSegs(seg, nseg)}, state,
+                       zero_grads, chan);
+}
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_fused_adamw_groups_kernel(CollDev d, size_t goff, size_t poff, size_t nvec,
+                                                                          const float* __restrict__ hp, const float4* __restrict__ groups,
+                                                                          int ngroups, const int4* __restrict__ seg, int nseg,
+                                                                          float* __restrict__ master, float* __restrict__ exp_avg,
+                                                                          float* __restrict__ exp_avg_sq, int zero_grads, int chan) {
+  __shared__ optim::AdamWCoef coef[BNET_GROUPS_MAX];
+  adamw_groups_coef(hp, groups, ngroups, coef);
+  float* const state[3] = {master, exp_avg, exp_avg_sq};
+  fused_step<DT, MODE>(d, HeapGrad{goff}, poff, nvec, AdamWGroupsOpt{coef[0], coef, GroupSegs(seg, nseg)}, state, zero_grads, chan);
+}
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_sgd_groups_kernel(CollDev d, size_t poff, size_t nvec,
+                                                                             const float* __restrict__ scratch, const float* __restrict__ clip,
+                                                                             const float* __restrict__ hp, const float4* __restrict__ groups,
+                                                                             int ngroups, const int4* __restrict__ seg, int nseg,
+                                                                             float* __restrict__ master, float* __restrict__ mom, int chan) {
+  __shared__ float2 grp[BNET_GROUPS_MAX];
+  sgd_groups_load(groups, ngroups, grp);
+  float* const state[2] = {master, mom};
+  fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec,
+                       SgdGroupsOpt<DT == BNET_BF16 ? 1 : 2>{hp[1], hp[3], grp, GroupSegs(seg, nseg)}, state, 0, chan);
+}
+
+template <int DT, int MODE>
+__global__ void __launch_bounds__(kThreads, 2) bnet_clip_apply_adamw_groups_kernel(CollDev d, size_t poff, size_t nvec,
+                                                                               const float* __restrict__ scratch, const float* __restrict__ clip,
+                                                                               const float* __restrict__ hp, const float4* __restrict__ groups,
+                                                                               int ngroups, const int4* __restrict__ seg, int nseg,
+                                                                               float* __restrict__ master, float* __restrict__ exp_avg,
+                                                                               float* __restrict__ exp_avg_sq, int chan) {
+  __shared__ optim::AdamWCoef coef[BNET_GROUPS_MAX];
+  adamw_groups_coef(hp, groups, ngroups, coef);
+  float* const state[3] = {master, exp_avg, exp_avg_sq};
+  fused_step<DT, MODE>(d, ScratchGrad{scratch, clip[optim::kClipCoef]}, poff, nvec, AdamWGroupsOpt{coef[0], coef, GroupSegs(seg, nseg)}, state,
+                       0, chan);
 }
 
 // ------------------------------------------------------------------ LARS: per-tensor trust ratios in the staged step
@@ -1669,6 +1807,80 @@ BNET_API int bnet_fused_clip_apply_adamw(BnetColl* c, size_t param_off, size_t c
                      stream, f) < 0)
     return -1;
   return run_fused_kernel<ClipAdamWKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, hp_dev, master, exp_avg, exp_avg_sq, channel);
+}
+
+// ---- parameter groups: the SGD and AdamW steps with per-group lr and weight decay (tables validated by the caller)
+struct SgdGroupsKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_fused_sgd_groups_kernel<DT, MODE>;
+};
+struct AdamWGroupsKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_fused_adamw_groups_kernel<DT, MODE>;
+};
+struct ClipSgdGroupsKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_clip_apply_sgd_groups_kernel<DT, MODE>;
+};
+struct ClipAdamWGroupsKernel {
+  template <int DT, int MODE> static constexpr auto fn = bnet_clip_apply_adamw_groups_kernel<DT, MODE>;
+};
+static_assert(sizeof(BnetGroupSeg) == sizeof(int4), "group segment rows are int4");
+
+static int groups_check(const float* hp_dev, const float* groups, int ngroups, const BnetGroupSeg* segs, int nseg) {
+  if (!hp_dev || ((uintptr_t)hp_dev & 15)) return fail("hyper-parameter block must be a 16-byte aligned device pointer");
+  if (ngroups < 1 || ngroups > BNET_GROUPS_MAX || !groups || ((uintptr_t)groups & 15))
+    return fail("group table needs 1..%d rows, 16-byte aligned (got %d)", BNET_GROUPS_MAX, ngroups);
+  if (nseg < 1 || !segs || ((uintptr_t)segs & 15)) return fail("group segment table needs >= 1 row, 16-byte aligned");
+  return 0;
+}
+
+BNET_API int bnet_fused_allreduce_sgd_groups(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype,
+                                             const float* hp_dev, const float* groups, int ngroups, const BnetGroupSeg* segs,
+                                             int nseg, float* master, float* mom_buf, int zero_grads, int channel, int nblocks,
+                                             void* stream) {
+  if (groups_check(hp_dev, groups, ngroups, segs, nseg) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "grouped SGD", grad_off, param_off, count, dtype, channel, {master, mom_buf}, nblocks, stream, f) < 0) return -1;
+  return run_fused<SgdGroupsKernel>(c, dtype, f, hp_dev, reinterpret_cast<const float4*>(groups), ngroups,
+                                    reinterpret_cast<const int4*>(segs), nseg, master, mom_buf, zero_grads, channel);
+}
+
+BNET_API int bnet_fused_allreduce_adamw_groups(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype,
+                                               const float* hp_dev, const float* groups, int ngroups, const BnetGroupSeg* segs,
+                                               int nseg, float* master, float* exp_avg, float* exp_avg_sq, int zero_grads,
+                                               int channel, int nblocks, void* stream) {
+  if (groups_check(hp_dev, groups, ngroups, segs, nseg) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "grouped AdamW", grad_off, param_off, count, dtype, channel, {master, exp_avg, exp_avg_sq}, nblocks, stream,
+                     f) < 0)
+    return -1;
+  return run_fused<AdamWGroupsKernel>(c, dtype, f, hp_dev, reinterpret_cast<const float4*>(groups), ngroups,
+                                      reinterpret_cast<const int4*>(segs), nseg, master, exp_avg, exp_avg_sq, zero_grads, channel);
+}
+
+BNET_API int bnet_fused_clip_apply_sgd_groups(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                              const float* clip, const float* hp_dev, const float* groups, int ngroups,
+                                              const BnetGroupSeg* segs, int nseg, float* master, float* mom_buf, int channel,
+                                              int nblocks, void* stream) {
+  if (groups_check(hp_dev, groups, ngroups, segs, nseg) < 0 || clip_block_check(clip) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "clipped grouped SGD", param_off, param_off, count, dtype, channel, {scratch, master, mom_buf}, nblocks,
+                     stream, f) < 0)
+    return -1;
+  return run_fused_kernel<ClipSgdGroupsKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, hp_dev, reinterpret_cast<const float4*>(groups),
+                                               ngroups, reinterpret_cast<const int4*>(segs), nseg, master, mom_buf, channel);
+}
+
+BNET_API int bnet_fused_clip_apply_adamw_groups(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                                const float* clip, const float* hp_dev, const float* groups, int ngroups,
+                                                const BnetGroupSeg* segs, int nseg, float* master, float* exp_avg,
+                                                float* exp_avg_sq, int channel, int nblocks, void* stream) {
+  if (groups_check(hp_dev, groups, ngroups, segs, nseg) < 0 || clip_block_check(clip) < 0) return -1;
+  FusedLaunch f;
+  if (fused_prologue(c, "clipped grouped AdamW", param_off, param_off, count, dtype, channel, {scratch, master, exp_avg, exp_avg_sq},
+                     nblocks, stream, f) < 0)
+    return -1;
+  return run_fused_kernel<ClipAdamWGroupsKernel>(c, dtype, f, f.poff, f.nvec, scratch, clip, hp_dev,
+                                                 reinterpret_cast<const float4*>(groups), ngroups, reinterpret_cast<const int4*>(segs),
+                                                 nseg, master, exp_avg, exp_avg_sq, channel);
 }
 
 // ---- LARS: norm, trust and apply stages (the tables themselves are validated by the caller before upload)

@@ -1,6 +1,7 @@
 // Per-element arithmetic of the fused optimizer kernels (csrc/cuda/coll.cu): sgd_update for
 // bnet_fused_sgd_kernel and adamw_update for bnet_fused_adamw_kernel, clip_coef for the clipped step, lars_trust /
-// lars_scalars for the LARS step, and ema_gate / ema_lerp for the EMA of the master weights.
+// lars_scalars for the LARS step, ema_gate / ema_lerp for the EMA of the master weights, and group_seg_find /
+// group_seg_advance, the parameter-group lookup of the grouped SGD and AdamW kernels.
 //
 // The updates are written here as plain __host__ __device__ functions so that the SAME code is (a) inlined into the
 // kernels by nvcc and (b) compiled by g++ (csrc/tests/optim_emu_test.cc checks SGD and AdamW against long-double
@@ -117,6 +118,30 @@ BNET_OPT_HD LarsScalars lars_scalars(float eta, float eps, float wd, float gs, f
 // The first four are the SGD block's {lr, momentum, weight_decay, grad_scale}.
 enum { kLarsLr = 0, kLarsMomentum, kLarsWeightDecay, kLarsGradScale, kLarsEta, kLarsEps, kLarsReserved0, kLarsReserved1,
        kLarsWords };
+
+// Parameter groups: the group table has one row of 4 floats per group, {lr, weight_decay, reserved, reserved}, and a
+// bucket's segment table per rank has int rows {vec0, nvec, group, reserved} (BnetGroupSeg), sorted by vec0, the first at
+// vector 0, covering the shard exactly once.  `seg` points at the first row's vec0; rows are 4 ints apart.  A shard has
+// fewer than 2^31 vectors (the host checks it), so vector indices are ints.
+enum { kGroupLr = 0, kGroupWeightDecay, kGroupReserved0, kGroupReserved1, kGroupWords };
+
+// The row holding shard vector v: the last row whose vec0 <= v (binary search; row 0 starts at 0).
+BNET_OPT_HD int group_seg_find(const int* seg, int nseg, int v) {
+  int lo = 0, hi = nseg - 1;
+  while (lo < hi) {
+    const int m = (lo + hi + 1) >> 1;
+    if (seg[4 * m] <= v) lo = m;
+    else hi = m - 1;
+  }
+  return lo;
+}
+
+// The same row, found by walking forward from row c, which holds a vector <= v.  A thread's vectors only increase, so a
+// cursor kept across them walks every row at most once in all.
+BNET_OPT_HD int group_seg_advance(const int* seg, int nseg, int c, int v) {
+  while (c + 1 < nseg && seg[4 * (c + 1)] <= v) ++c;
+  return c;
+}
 
 // Device block of the exponential moving average of the master weights: 4 floats, 16-byte aligned.  `weight` is
 // 1 - decay, computed in double by the host and rounded once, which is the fp32 weight torch._foreach_lerp_ gets from

@@ -7,7 +7,7 @@ import os
 import torch
 
 from bagua_net_b200.models import build_model
-from bagua_net_b200.parallel import BnetDDP, init_process_group_from_env
+from bagua_net_b200.parallel import BnetDDP, init_process_group_from_env, no_weight_decay_groups
 
 
 def batches(n, batch, device_rank):
@@ -26,6 +26,8 @@ def main():
     ap.add_argument("--ema-decay", type=float, default=None,
                     help="keep an exponential moving average of the weights with this decay (torchvision uses 0.99998)")
     ap.add_argument("--ema-every", type=int, default=1, help="update the EMA after every this many optimizer steps")
+    ap.add_argument("--no-decay-1d", action="store_true",
+                    help="no weight decay on biases and normalisation weights (torchvision's --norm-weight-decay 0.0)")
     ap.add_argument("--model", default="vgg16")
     ap.add_argument("--checkpoint", default="")
     a = ap.parse_args()
@@ -33,7 +35,8 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     model = build_model(a.model, fused=True).cuda().bfloat16().to(memory_format=torch.channels_last)
     engine = BnetDDP(model, lr=0.01, momentum=0.9, weight_decay=1e-4, accumulation_steps=a.accumulation_steps,
-                     ema_decay=a.ema_decay, ema_every=a.ema_every)
+                     ema_decay=a.ema_decay, ema_every=a.ema_every,
+                     param_groups=no_weight_decay_groups(model) if a.no_decay_1d else None)
     engine.enable_cuda_graph(True)            # forward + backward + every bucket kernel replay as one graph
     engine.set_lr(0.01)                       # hyper-parameters live in device memory: the graph follows the schedule
     last = []

@@ -175,6 +175,40 @@ int bnet_fused_lars_apply(BnetColl* c, size_t param_off, size_t count, int dtype
                           int nseg, const float* scal, const float* hp, float* master, float* mom_buf, int channel, int nblocks,
                           void* stream);
 
+/* Parameter groups: the SGD and AdamW steps with a learning rate and weight decay per group of parameter tensors, as
+ * torch.optim's param groups.  The group table is `ngroups` rows of 4 floats of device memory, 16-byte aligned:
+ * {lr, weight_decay, reserved, reserved} (csrc/cuda/optim_body.cuh), read when the kernel runs, so a captured CUDA graph
+ * follows changes to it; 1 <= ngroups <= BNET_GROUPS_MAX.
+ *
+ * A group segment is a run of consecutive shard vectors of one group: `nvec` 16-byte vectors from shard vector `vec0`.
+ * A bucket's table per rank lists them sorted by vec0 and covers the shard exactly once; every tensor starts on a 16-byte
+ * boundary, so no vector holds two tensors, and zero padding joins a neighbouring segment.  The caller validates the
+ * table (group indices below ngroups included) before it uploads it: the kernels trust it. */
+#define BNET_GROUPS_MAX 64
+typedef struct {
+  int32_t vec0, nvec, group, reserved;
+} BnetGroupSeg;
+/* bnet_fused_allreduce_sgd_hp with every vector's lr and weight decay taken from its group's row: the momentum and
+ * grad_scale come from the 4-float SGD block hp_dev, whose lr and weight_decay are not read.  A group with weight decay 0
+ * skips the decay term, as torch does. */
+int bnet_fused_allreduce_sgd_groups(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, const float* hp_dev,
+                                    const float* groups, int ngroups, const BnetGroupSeg* segs, int nseg, float* master,
+                                    float* mom_buf, int zero_grads, int channel, int nblocks, void* stream);
+/* bnet_fused_allreduce_adamw with every vector's lr and weight decay taken from its group's row; betas, eps, grad_scale and
+ * step come from the 8-float AdamW block hp_dev, whose lr and weight_decay are not read.  A group's elements get the bits
+ * the ungrouped kernel gives them with the group's lr and weight decay in the block. */
+int bnet_fused_allreduce_adamw_groups(BnetColl* c, size_t grad_off, size_t param_off, size_t count, int dtype, const float* hp_dev,
+                                      const float* groups, int ngroups, const BnetGroupSeg* segs, int nseg, float* master,
+                                      float* exp_avg, float* exp_avg_sq, int zero_grads, int channel, int nblocks, void* stream);
+/* Stage 3 of the staged step with groups: bnet_fused_clip_apply_sgd_hp / _adamw with the per-group values as above. */
+int bnet_fused_clip_apply_sgd_groups(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch, const float* clip,
+                                     const float* hp_dev, const float* groups, int ngroups, const BnetGroupSeg* segs, int nseg,
+                                     float* master, float* mom_buf, int channel, int nblocks, void* stream);
+int bnet_fused_clip_apply_adamw_groups(BnetColl* c, size_t param_off, size_t count, int dtype, const float* scratch,
+                                       const float* clip, const float* hp_dev, const float* groups, int ngroups,
+                                       const BnetGroupSeg* segs, int nseg, float* master, float* exp_avg, float* exp_avg_sq,
+                                       int channel, int nblocks, void* stream);
+
 /* Exponential moving average (EMA) of the fp32 master weights, as torch.optim.swa_utils.AveragedModel with
  * get_ema_multi_avg_fn(decay) and use_buffers=False, applied to this rank's master shards.  The EMA block is 4 floats of
  * device memory, 16-byte aligned: {weight = 1 - decay, every, step, n_averaged} (csrc/cuda/optim_body.cuh).  `step`
