@@ -285,7 +285,13 @@ class SymmComm:
 
     def all_reduce_oneshot(self, t: torch.Tensor, out: torch.Tensor, op: str = "sum", channel: int = 1,
                            nblocks: int = 0, stream=None) -> torch.Tensor:
+        """Out-of-place all-reduce: every rank reads every rank's heap tensor ``t`` and writes the result to its own
+        ``out`` (any CUDA memory).  ``out`` must not overlap ``t``: peers may still be reading ``t`` while this rank
+        writes ``out``."""
         assert out.is_contiguous() and out.numel() == t.numel() and out.dtype == t.dtype
+        nbytes = t.numel() * t.element_size()
+        if out.data_ptr() < t.data_ptr() + nbytes and t.data_ptr() < out.data_ptr() + nbytes:
+            raise ValueError("all_reduce_oneshot is out of place: `out` overlaps `t`, which the peers are still reading")
         n = self._chk(self.lib.bnet_allreduce_oneshot(self.h, self.offset_of(t), C.c_void_p(out.data_ptr()), t.numel(),
                                                       DT[t.dtype], OPS[op], channel, nblocks, self._stream(stream)),
                       "all_reduce_oneshot")

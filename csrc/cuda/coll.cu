@@ -139,31 +139,18 @@ __device__ __forceinline__ float combine(float a, float b) {
 }
 
 // in-switch reduction of one 16-byte vector across all ranks bound to the multicast object
+// (add only: max and min take the peer-load kernel, see run_allreduce_op)
 template <int DT, int OP>
 __device__ __forceinline__ int4 mc_ld_reduce(const char* p) {
+  static_assert(OP == BNET_SUM || OP == BNET_AVG, "the in-switch reduction is used for add only");
   int4 r;
   if constexpr (DT == BNET_F32) {
-    static_assert(OP == BNET_SUM || OP == BNET_AVG, "multimem f32 supports add only");
     float4 f = ptx::multimem_ld_reduce_add_f32x4(p);
     r.x = __float_as_int(f.x); r.y = __float_as_int(f.y); r.z = __float_as_int(f.z); r.w = __float_as_int(f.w);
   } else if constexpr (DT == BNET_BF16) {
-    if constexpr (OP == BNET_MAX)
-      asm volatile("multimem.ld_reduce.relaxed.sys.global.max.v4.bf16x2 {%0,%1,%2,%3}, [%4];"
-                   : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
-    else if constexpr (OP == BNET_MIN)
-      asm volatile("multimem.ld_reduce.relaxed.sys.global.min.v4.bf16x2 {%0,%1,%2,%3}, [%4];"
-                   : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
-    else
-      r = ptx::multimem_ld_reduce_add_bf16x8(p);
+    r = ptx::multimem_ld_reduce_add_bf16x8(p);
   } else {
-    if constexpr (OP == BNET_MAX)
-      asm volatile("multimem.ld_reduce.relaxed.sys.global.max.v4.f16x2 {%0,%1,%2,%3}, [%4];"
-                   : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
-    else if constexpr (OP == BNET_MIN)
-      asm volatile("multimem.ld_reduce.relaxed.sys.global.min.v4.f16x2 {%0,%1,%2,%3}, [%4];"
-                   : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
-    else
-      r = ptx::multimem_ld_reduce_add_f16x8(p);
+    r = ptx::multimem_ld_reduce_add_f16x8(p);
   }
   return r;
 }
@@ -435,6 +422,8 @@ __device__ __forceinline__ void fused_grad_issue(const CollDev& d, size_t go, in
   else if constexpr (MODE == 2) p2p_reduce<DT, BNET_SUM>(d, go, d.rank, gf);
   else gv = ptx::ld_na_v4(reinterpret_cast<const int4*>(d.heap[0] + go));
 }
+// ... as fp32 lanes.  For bf16 gradients the modes differ before the fp32 update: MODE 1 gets the switch's sum
+// rounded to bf16 (the switch returns the dtype), MODE 2 keeps the fp32 sum of the peer loads.
 template <int DT, int MODE>
 __device__ __forceinline__ void fused_grad_get(const int4& gv, const float* gf, float* g) {
   if constexpr (MODE == 2) {
@@ -1536,12 +1525,11 @@ static int run_allreduce_op(BnetColl* c, int op, int algo, size_t off, size_t nv
   switch (op) {
     case BNET_SUM: return run_allreduce<DT, BNET_SUM>(c, algo, off, nvec, chan, nb, st);
     case BNET_AVG: return run_allreduce<DT, BNET_AVG>(c, algo, off, nvec, chan, nb, st);
-    case BNET_MAX:
-      if constexpr (DT == BNET_F32) { if (algo == BNET_ALGO_NVLS) algo = BNET_ALGO_P2P_TWOSHOT; return launch(bnet_allreduce_p2p_kernel<DT, BNET_MAX>, nb, kThreads, st, c->devp, off, nvec, chan); }
-      else return run_allreduce<DT, BNET_MAX>(c, algo, off, nvec, chan, nb, st);
-    case BNET_MIN:
-      if constexpr (DT == BNET_F32) { return launch(bnet_allreduce_p2p_kernel<DT, BNET_MIN>, nb, kThreads, st, c->devp, off, nvec, chan); }
-      else return run_allreduce<DT, BNET_MIN>(c, algo, off, nvec, chan, nb, st);
+    // max and min never use the switch, whatever `algo` asks: the peer-load, one-shot and LL kernels all combine with
+    // fmaxf / fminf (a NaN loses to a number), and multimem's min / max has no f32 form and no
+    // documented NaN rule, so a result's NaNs would depend on the dtype, the world size and the message size.
+    case BNET_MAX: return launch(bnet_allreduce_p2p_kernel<DT, BNET_MAX>, nb, kThreads, st, c->devp, off, nvec, chan);
+    case BNET_MIN: return launch(bnet_allreduce_p2p_kernel<DT, BNET_MIN>, nb, kThreads, st, c->devp, off, nvec, chan);
   }
   return fail("bad op %d", op);
 }
@@ -1586,6 +1574,7 @@ BNET_API int bnet_allreduce_oneshot(BnetColl* c, size_t offset, void* out, size_
   if (channel < 0 || channel >= BNET_COLL_CHANNELS) return fail("bad channel");
   size_t bytes = count * elsize(dtype);
   if (bytes % 16 || offset % 16 || ((uintptr_t)out & 15)) return fail("one-shot all-reduce needs 16-byte alignment");
+  if (offset + bytes > c->alloc_bytes - kPadBytes) return fail("one-shot all-reduce range outside the heap");
   refresh_devp(c);
   size_t nvec = bytes / 16;
   int nb = pick_blocks(c, nvec, nblocks, BLK_P2P);

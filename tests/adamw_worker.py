@@ -101,12 +101,16 @@ class Reference:
 
 # ------------------------------------------------------------------ the kernel against float64
 def grads_for(step, n, dtype, scale=1.0):
-    """Every rank's gradient of `step`: multiples of 2^-6 in [-1, 1], so the sum over ranks is exact in bf16 and fp32
-    whichever way the kernel reduces (in the switch, with peer loads, or locally)."""
+    """Every rank's gradient of `step`: multiples of 2^-q in [-1, 1] with q = 6 up to four ranks and
+    q = 8 - ceil(log2 WORLD) above, so that every partial sum over the ranks is a multiple of 2^-q of magnitude at most
+    WORLD * 2^q <= 2^8: exact in bf16 (8 significant bits) and fp32 whichever way and in whatever order the kernel reduces
+    (in the switch, which rounds its sum to bf16, with peer loads in fp32, or locally).  With q = 6 at eight ranks a sum
+    could reach 512 and need 9 bits; up to four ranks the data is the same as with q = 6 everywhere."""
+    q = 64 if WORLD <= 4 else 2 ** (8 - math.ceil(math.log2(WORLD)))
     gs = []
     for r in range(WORLD):
         gen = torch.Generator(device="cuda").manual_seed(1000 * step + r)
-        gs.append((torch.randint(-64, 65, (n,), device="cuda", generator=gen).float() / 64 * scale).to(dtype))
+        gs.append((torch.randint(-q, q + 1, (n,), device="cuda", generator=gen).float() / q * scale).to(dtype))
     return gs
 
 
