@@ -1,13 +1,15 @@
 """What the CPU tests of BnetDDP's host logic put in place of the GPU: a comm that does every SymmComm call the engine
 makes with the same arithmetic in plain PyTorch (one rank, host memory), stubs for the CUDA stream / event calls (the
-`cpu_engine` fixture) and a small model.  bagua_net_b200/parallel/ddp.py itself runs unmodified."""
+`cpu_engine` fixture) and a small model.  bagua_net_b200/parallel/ddp.py itself runs unmodified.  Also the torch side
+the engine is trained against: the hyper-parameters, an engine / torch.optim pair, the batches and the reference step."""
 import contextlib
 import math
 
 import pytest
 import torch
 
-from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_lars_segments, check_lars_tensors
+from bagua_net_b200.parallel.comm import CLIP_ROW, LARS_CHUNK, check_group_segments, check_lars_segments, check_lars_tensors
+from bagua_net_b200.parallel.ddp import BnetDDP
 
 
 class FakeStream:
@@ -31,9 +33,9 @@ class FakeComm:
     assert the argument contracts that SymmComm enforces on the engine's calls.  `log` lists every call in order as
     (kind, size):
 
-    sgd / adamw (one-kernel step) and norm / accum (stage 1): the gradient numel;  coef: the number of partial rows;
-    barrier: None;  apply (stage-3 SGD / AdamW) and lars_apply: the param numel;  lars_norm and ema_update: the master
-    numel;  lars_trust: the number of tensors;  ema_advance: None."""
+    sgd / adamw / sgd_groups / adamw_groups (one-kernel step) and norm / accum (stage 1): the gradient numel;  coef: the
+    number of partial rows;  barrier: None;  apply / apply_groups (stage-3 SGD / AdamW) and lars_apply: the param numel;
+    lars_norm and ema_update: the master numel;  lars_trust: the number of tensors;  ema_advance: None."""
 
     def __init__(self):
         self.world, self.rank, self.launches = 1, 0, 0
@@ -42,15 +44,16 @@ class FakeComm:
         self.coef_scales = []              # the gradient scale of every coefficient launch
         self.apply_scales = []             # ... and of every SGD / AdamW update from the scratch
         self._lars_nslots = {}             # id of a segment table from lars_segments -> (the table, its norm slots)
+        self._group_tables = {}            # id of a segment table from group_segments -> (shard vectors, groups)
 
     def _launched(self, kind, size):
         self.launches += 1
         self.log.append((kind, size))
 
-    def alloc(self, numel, dtype):
+    def alloc(self, numel, dtype, align=256):
         return torch.zeros(numel, dtype=dtype)
 
-    def all_reduce(self, t, op="sum", **kw):
+    def all_reduce(self, t, op="sum", algo="auto", channel=1, nblocks=0, stream=None):
         return t
 
     def barrier(self, channel=2, stream=None):
@@ -137,6 +140,57 @@ class FakeComm:
         self.apply_scales.append(self._adamw(scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp))
         self._launched("apply", param.numel())
 
+    # ------------------------------------------------------------------ parameter groups: each segment of the validated
+    # table updated with its group's row
+    def group_segments(self, table, shard_vecs, ngroups):
+        check_group_segments(table, shard_vecs, ngroups)
+        t = torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
+        self._group_tables[id(t)] = (shard_vecs, ngroups)
+        return t
+
+    def _per_segment(self, param, segs, groups, hp, update):
+        shard_vecs, ngroups = self._group_tables[id(segs)]
+        e = 16 // param.element_size()
+        assert shard_vecs * e == param.numel() and groups.shape == (groups.shape[0], 4) and groups.shape[0] >= ngroups
+        for vec0, nvec, g, _ in segs.tolist():
+            h = hp.clone()
+            h[0], h[4 if hp.numel() == 8 else 2] = groups[g, 0], groups[g, 1]
+            update(slice(vec0 * e, (vec0 + nvec) * e), h)
+
+    def _sgd_groups(self, g, param, master, mom, hp, groups, segs):
+        assert hp.numel() == 4
+        self._per_segment(param, segs, groups, hp, lambda s, h: self._sgd(g[s], param[s], master[s], mom[s], 0, 0, 0, None, h))
+        return float(hp[3])
+
+    def _adamw_groups(self, g, param, master, exp_avg, exp_avg_sq, hp, groups, segs):
+        steps = len(self.steps_seen)
+        self._per_segment(param, segs, groups, hp,
+                          lambda s, h: self._adamw(g[s], param[s], master[s], exp_avg[s], exp_avg_sq[s], h))
+        del self.steps_seen[steps + 1:]    # (one step, however many segments)
+        return float(hp[5])
+
+    def fused_allreduce_sgd_groups(self, grad, param, master, mom, hp, groups, segs, zero_grads=True, channel=0, nblocks=0,
+                                   stream=None):
+        self._sgd_groups(grad, param, master, mom, hp, groups, segs)
+        grad.zero_()
+        self._launched("sgd_groups", grad.numel())
+
+    def fused_allreduce_adamw_groups(self, grad, param, master, exp_avg, exp_avg_sq, hp, groups, segs, zero_grads=True,
+                                     channel=0, nblocks=0, stream=None):
+        self._adamw_groups(grad, param, master, exp_avg, exp_avg_sq, hp, groups, segs)
+        grad.zero_()
+        self._launched("adamw_groups", grad.numel())
+
+    def fused_clip_apply_sgd_groups(self, param, scratch, clip, master, mom, hp, groups, segs, channel=0, nblocks=0,
+                                    stream=None):
+        self.apply_scales.append(self._sgd_groups(scratch * clip[2], param, master, mom, hp, groups, segs))
+        self._launched("apply_groups", param.numel())
+
+    def fused_clip_apply_adamw_groups(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, groups, segs, channel=0,
+                                      nblocks=0, stream=None):
+        self.apply_scales.append(self._adamw_groups(scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, groups, segs))
+        self._launched("apply_groups", param.numel())
+
     # ------------------------------------------------------------------ LARS: norm, trust, apply
     def lars_segments(self, table, shard_vecs, ntensors):
         t = torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
@@ -212,3 +266,84 @@ def small_model(channels_last=True):
     m = torch.nn.Sequential(torch.nn.Conv2d(3, 8, 3, padding=1), torch.nn.ReLU(), torch.nn.Conv2d(8, 8, 3, padding=1), torch.nn.ReLU(),
                             torch.nn.AdaptiveAvgPool2d(2), torch.nn.Flatten(), torch.nn.Linear(32, 10))
     return m.to(memory_format=torch.channels_last) if channels_last else m
+
+
+class Branchy(torch.nn.Module):
+    """small_model plus layers that fill a bucket each, registered first: `unused` never gets a gradient, `late` (built
+    when asked) only while `use_late` is on."""
+
+    def __init__(self, channels_last=True, late=False):
+        super().__init__()
+        torch.manual_seed(4)
+        self.unused = torch.nn.Linear(32, 32, bias=False)
+        if late:
+            self.late = torch.nn.Linear(32, 32, bias=False)
+        self.net = small_model(channels_last)
+        self.use_late = False
+
+    def forward(self, x):
+        h = self.net[:-1](x)
+        if self.use_late:
+            h = h + self.late(h)
+        return self.net[-1](h)
+
+
+# ------------------------------------------------------------------ the torch side
+LARC = dict(weight_decay=5e-4, trust_coefficient=0.02, eps=1e-8)
+HYPER = {"sgd": dict(lr=0.05, momentum=0.9, weight_decay=1e-3),
+         "adamw": dict(lr=3e-3, betas=(0.85, 0.99), eps=1e-7, weight_decay=0.05),
+         "lars": dict(lr=0.5, momentum=0.9, **LARC)}
+
+
+def make_pair(optimizer, model=small_model, channels_last=True, dtype=torch.float64, **engine_kw):
+    """(torch reference in `dtype`, its torch.optim optimizer, the engine's model, the engine with ~2 KB buckets): both
+    from `model(channels_last)` and HYPER[optimizer].  LARS's reference optimizer is SGD without weight decay: larc_
+    applies it."""
+    ref, net = model(channels_last).to(dtype), model(channels_last)
+    h = HYPER[optimizer]
+    if optimizer == "adamw":
+        opt = torch.optim.AdamW(ref.parameters(), **h)
+    else:
+        opt = torch.optim.SGD(ref.parameters(), lr=h["lr"], momentum=h["momentum"],
+                              weight_decay=0.0 if optimizer == "lars" else h["weight_decay"])
+    eng = BnetDDP(net, optimizer=optimizer, bucket_mb=0.002, comm=FakeComm(), **h, **engine_kw)
+    return ref, opt, net, eng
+
+
+def batch(step, n, seed, channels_last=True):
+    torch.manual_seed(seed + step)
+    x, y = torch.randn(n, 3, 8, 8), torch.randint(0, 10, (n,))
+    return (x.contiguous(memory_format=torch.channels_last) if channels_last else x), y
+
+
+def larc_(params, weight_decay, trust_coefficient, eps):
+    """NVIDIA Apex LARC(clip=False) on the .grad of `params`: weight decay and the trust ratio folded into the gradient
+    of every tensor of more than one dimension that has one."""
+    with torch.no_grad():
+        for p in params:
+            if p.grad is None or p.dim() <= 1:
+                continue
+            wn, gn = p.norm(), p.grad.norm()
+            if wn != 0 and gn != 0:
+                t = trust_coefficient * wn / (gn + wn * weight_decay + eps)
+                p.grad.add_(p, alpha=weight_decay).mul_(t)
+
+
+def torch_step(ref, opt, x, y, k=1, max_norm=None, lars=None) -> float:
+    """One optimizer step of the torch reference on the batch: k equal micro-batches accumulated as loss / k each,
+    clip_grad_norm_ to `max_norm` (None: inf, which multiplies the gradients by exactly 1), Apex LARC with
+    `lars` = dict(weight_decay, trust_coefficient, eps), then `opt`.  Returns the pre-clip gradient norm."""
+    opt.zero_grad()
+    dtype = next(ref.parameters()).dtype
+    for xs, ys in zip(x.chunk(k), y.chunk(k)):
+        (torch.nn.functional.cross_entropy(ref(xs.to(dtype)), ys) / k).backward()
+    norm = torch.nn.utils.clip_grad_norm_(ref.parameters(), math.inf if max_norm is None else max_norm)
+    if lars is not None:
+        larc_(ref.parameters(), **lars)
+    opt.step()
+    return float(norm)
+
+
+def close_params(net, ref, atol, tag=None, rtol=0.0):
+    for a, b in zip(net.parameters(), ref.parameters()):
+        assert torch.allclose(a.to(b.dtype), b, rtol=rtol, atol=atol), (tag, float((a.to(b.dtype) - b).abs().max()))

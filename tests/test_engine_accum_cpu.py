@@ -10,51 +10,15 @@ import math
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import Branchy, batch, close_params, make_pair, torch_step
 from engine_fakes import small_model as _model
 
 from bagua_net_b200.parallel.ddp import BnetDDP
 
 
 BATCH = 12                                      # divisible by every k tested
-
-
-def _batch(step, channels_last=True, n=BATCH):
-    torch.manual_seed(100 + step)
-    x, y = torch.randn(n, 3, 8, 8), torch.randint(0, 10, (n,))
-    return (x.contiguous(memory_format=torch.channels_last) if channels_last else x), y
-
-
-SGD = dict(lr=0.05, momentum=0.9, weight_decay=1e-3)
-ADAMW = dict(lr=3e-3, betas=(0.85, 0.99), eps=1e-7, weight_decay=0.05)
 # clipping thresholds per step: far below the gradient norm, far above it, inf (norm only), below again
 THRESHOLDS = [1e-2, 1e3, math.inf, 1e-2]
-
-
-def _pair(optimizer, channels_last=True, model=None, **kw):
-    """(float64 torch reference, its optimizer, the engine's model, the engine)."""
-    make = model or _model
-    ref, net = make(channels_last).double(), make(channels_last)
-    if optimizer == "adamw":
-        opt = torch.optim.AdamW(ref.parameters(), **ADAMW)
-        eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=FakeComm(), **ADAMW, **kw)
-    else:
-        opt = torch.optim.SGD(ref.parameters(), **SGD)
-        eng = BnetDDP(net, bucket_mb=0.002, comm=FakeComm(), **SGD, **kw)
-    return ref, opt, net, eng
-
-
-def _torch_step(ref, opt, x, y, max_norm):
-    """One step on the full batch in float64; returns the pre-clip norm of the mean gradient."""
-    opt.zero_grad()
-    torch.nn.functional.cross_entropy(ref(x.double()), y).backward()
-    norm = torch.nn.utils.clip_grad_norm_(ref.parameters(), max_norm if max_norm is not None else math.inf)
-    opt.step()
-    return float(norm)
-
-
-def _close(net, ref, step):
-    for a, b in zip(net.parameters(), ref.parameters()):
-        assert torch.allclose(a.double(), b, rtol=0, atol=2e-5), (step, float((a.double() - b).abs().max()))
 
 
 @pytest.mark.parametrize("k", [2, 3, 4])
@@ -65,8 +29,8 @@ def _close(net, ref, step):
 def test_accumulating_engine_trains_like_torch_on_the_full_batch(cpu_engine, k, optimizer, clipped, direct_grads,
                                                                  channels_last):
     cpu_engine.setenv("BNET_DIRECT_GRADS", direct_grads)
-    ref, opt, net, eng = _pair(optimizer, channels_last, max_grad_norm=THRESHOLDS[0] if clipped else None,
-                               accumulation_steps=k)
+    ref, opt, net, eng = make_pair(optimizer, channels_last=channels_last, max_grad_norm=THRESHOLDS[0] if clipped else None,
+                                   accumulation_steps=k)
     assert len(eng.buckets) >= 2 and eng.accumulation_steps == k
     for step, thr in enumerate(THRESHOLDS):
         if clipped and thr != eng.max_grad_norm:
@@ -76,8 +40,8 @@ def test_accumulating_engine_trains_like_torch_on_the_full_batch(cpu_engine, k, 
             eng.set_lr(lr)                                       # scalar launch arguments -> the device block
             for g in opt.param_groups:
                 g["lr"] = lr
-        x, y = _batch(step, channels_last)
-        want = _torch_step(ref, opt, x, y, thr if clipped else None)
+        x, y = batch(step, BATCH, 100, channels_last)
+        want = torch_step(ref, opt, x, y, max_norm=thr if clipped else None)     # on the full batch
         eng.train_step(x, y)
         assert eng.micro_step == 0
         if clipped:
@@ -85,7 +49,7 @@ def test_accumulating_engine_trains_like_torch_on_the_full_batch(cpu_engine, k, 
         else:
             assert eng.last_grad_norm is None
         assert float(eng.flat_grad.abs().max()) == 0.0
-        _close(net, ref, step)
+        close_params(net, ref, 2e-5, step)
     scales = eng.comm.apply_scales
     assert scales and all(s == pytest.approx(1.0 / k) for s in scales)
     if clipped:
@@ -93,8 +57,8 @@ def test_accumulating_engine_trains_like_torch_on_the_full_batch(cpu_engine, k, 
 
 
 def test_train_step_loss_is_the_mean_of_the_micro_batch_losses(cpu_engine):
-    ref, opt, net, eng = _pair("sgd", accumulation_steps=3)
-    x, y = _batch(0)
+    ref, opt, net, eng = make_pair("sgd", accumulation_steps=3)
+    x, y = batch(0, BATCH, 100)
     with torch.no_grad():
         want = sum(float(torch.nn.functional.cross_entropy(net(xs), ys)) for xs, ys in zip(x.split(4), y.split(4))) / 3
     assert float(eng.train_step(x, y)) == pytest.approx(want, rel=1e-6)
@@ -104,12 +68,12 @@ def test_train_step_loss_is_the_mean_of_the_micro_batch_losses(cpu_engine):
 @pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
 def test_launch_log_per_micro_batch_and_per_step(cpu_engine, optimizer, clipped):
     k = 3
-    ref, opt, net, eng = _pair(optimizer, max_grad_norm=1.0 if clipped else None, accumulation_steps=k)
+    ref, opt, net, eng = make_pair(optimizer, max_grad_norm=1.0 if clipped else None, accumulation_steps=k)
     comm, nb = eng.comm, len(eng.buckets)
     sizes = sorted(b.numel for b in eng.buckets)
     for step in range(2):
         n0, l0 = len(comm.log), comm.launches
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, BATCH, 100))
         log = comm.log[n0:]
         stage2 = "coef" if clipped else "barrier"
         assert [kind for kind, _ in log] == ["norm"] * nb + ["accum"] * nb * (k - 1) + [stage2] + ["apply"] * nb
@@ -128,9 +92,9 @@ def test_one_micro_batch_keeps_the_old_step(cpu_engine, optimizer, clipped):
     """accumulation_steps=1 issues exactly the calls an engine without the argument issues, with the same scales."""
     logs = []
     for kw in ({}, {"accumulation_steps": 1}):
-        ref, opt, net, eng = _pair(optimizer, max_grad_norm=0.5 if clipped else None, **kw)
+        ref, opt, net, eng = make_pair(optimizer, max_grad_norm=0.5 if clipped else None, **kw)
         for step in range(2):
-            eng.train_step(*_batch(step, n=4))
+            eng.train_step(*batch(step, 4, 100))
         logs.append((eng.comm.log, eng.comm.coef_scales, eng.comm.apply_scales, [p.detach().clone() for p in net.parameters()]))
         nb = len(eng.buckets)
         if clipped:
@@ -142,31 +106,13 @@ def test_one_micro_batch_keeps_the_old_step(cpu_engine, optimizer, clipped):
     assert all(torch.equal(a, b) for a, b in zip(logs[0][3], logs[1][3]))
 
 
-class _Branchy(torch.nn.Module):
-    """small_model plus two layers that fill a bucket each: `late` is used only when switched on, `unused` never."""
-
-    def __init__(self, channels_last=True):
-        super().__init__()
-        torch.manual_seed(4)
-        self.unused = torch.nn.Linear(32, 32, bias=False)
-        self.late = torch.nn.Linear(32, 32, bias=False)
-        self.net = _model(channels_last)
-        self.use_late = False
-
-    def forward(self, x):
-        h = self.net[:-1](x)
-        if self.use_late:
-            h = h + self.late(h)
-        return self.net[-1](h)
-
-
 @pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
 def test_bucket_first_fed_in_the_second_micro_batch_stores_and_an_idle_bucket_is_left_alone(cpu_engine, clipped):
     """A custom backward + finish_step loop; the reference is torch's own accumulation (loss / k per micro-batch) in float64.
     `late` gets its first gradient in micro-batch 2 (stored, not added to a stale scratch), `unused` none in the step
     (no update, nothing in the norm)."""
     k, thr = 3, (0.05 if clipped else None)
-    ref, opt, net, eng = _pair("sgd", model=_Branchy, max_grad_norm=thr, accumulation_steps=k)
+    ref, opt, net, eng = make_pair("sgd", model=lambda cl: Branchy(cl, late=True), max_grad_norm=thr, accumulation_steps=k)
     late = [b for b in eng.buckets if len(b.params) == 1 and b.params[0] is net.late.weight]
     idle = [b for b in eng.buckets if len(b.params) == 1 and b.params[0] is net.unused.weight]
     assert len(late) == 1 and len(idle) == 1
@@ -174,7 +120,7 @@ def test_bucket_first_fed_in_the_second_micro_batch_stores_and_an_idle_bucket_is
     w0 = net.unused.weight.detach().clone()
     late.scratch.fill_(1e6)                                      # stale: must be overwritten, not added to
     for step in range(3):
-        x, y = _batch(step)
+        x, y = batch(step, BATCH, 100)
         opt.zero_grad()
         n0 = len(eng.comm.log)
         for m, (xs, ys) in enumerate(zip(x.split(BATCH // k), y.split(BATCH // k))):
@@ -189,7 +135,7 @@ def test_bucket_first_fed_in_the_second_micro_batch_stores_and_an_idle_bucket_is
         assert late_calls == ["norm", "accum"]                   # micro-batch 2 stores, micro-batch 3 adds
         if clipped:
             assert float(eng.last_grad_norm) == pytest.approx(want, rel=1e-5)
-        _close(net, ref, step)
+        close_params(net, ref, 2e-5, step)
     assert torch.equal(net.unused.weight, w0)
     assert [kind for kind, _ in eng.comm.log].count("apply") == 3 * (len(eng.buckets) - 1)
     assert float(idle.partial.abs().max()) == 0.0
@@ -198,10 +144,10 @@ def test_bucket_first_fed_in_the_second_micro_batch_stores_and_an_idle_bucket_is
 @pytest.mark.parametrize("optimizer", ["sgd", "adamw"])
 def test_custom_loop_matches_train_step(cpu_engine, optimizer):
     k = 4
-    a = _pair(optimizer, max_grad_norm=0.1, accumulation_steps=k)
-    b = _pair(optimizer, max_grad_norm=0.1, accumulation_steps=k)
+    a = make_pair(optimizer, max_grad_norm=0.1, accumulation_steps=k)
+    b = make_pair(optimizer, max_grad_norm=0.1, accumulation_steps=k)
     for step in range(3):
-        x, y = _batch(step)
+        x, y = batch(step, BATCH, 100)
         a[3].train_step(x, y)
         for m, (xs, ys) in enumerate(zip(x.split(BATCH // k), y.split(BATCH // k))):
             assert b[3].micro_step == m
@@ -218,13 +164,13 @@ def test_custom_loop_matches_train_step(cpu_engine, optimizer):
 
 @pytest.mark.parametrize("optimizer", ["sgd", "adamw"])
 def test_checkpoint_at_step_boundaries_only(cpu_engine, optimizer):
-    ref, opt, net, eng = _pair(optimizer, accumulation_steps=2)
-    plain = _pair(optimizer)[3]
-    eng.train_step(*_batch(0))
+    ref, opt, net, eng = make_pair(optimizer, accumulation_steps=2)
+    plain = make_pair(optimizer)[3]
+    eng.train_step(*batch(0, BATCH, 100))
     state = eng.optimizer_state_dict()
     assert set(state) == set(plain.optimizer_state_dict())
     assert [set(s) for s in state["buckets"]] == [set(s) for s in plain.optimizer_state_dict()["buckets"]]
-    x, y = _batch(1)
+    x, y = batch(1, BATCH, 100)
     torch.nn.functional.cross_entropy(net(x[:6]), y[:6]).backward()
     eng.finish_step()
     assert eng.micro_step == 1
@@ -237,7 +183,7 @@ def test_checkpoint_at_step_boundaries_only(cpu_engine, optimizer):
     torch.nn.functional.cross_entropy(net(x[6:]), y[6:]).backward()
     eng.finish_step()
     assert eng.micro_step == 0
-    resumed = _pair(optimizer, accumulation_steps=2)[3]
+    resumed = make_pair(optimizer, accumulation_steps=2)[3]
     resumed.load_optimizer_state_dict(copy.deepcopy(eng.optimizer_state_dict()))
     for b1, b2 in zip(resumed.buckets, eng.buckets):
         assert all(torch.equal(t1, t2) for t1, t2 in zip(b1.state, b2.state))
@@ -249,10 +195,10 @@ def test_rejects_bad_arguments(cpu_engine):
             BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=bad)
     eng = BnetDDP(_model(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=4)
     for n in (6, 10, 3):
-        x, y = _batch(0, n=n)
+        x, y = batch(0, n, 100)
         with pytest.raises(ValueError):
             eng.train_step(x, y)
-    x, y = _batch(0, n=8)
+    x, y = batch(0, 8, 100)
     with pytest.raises(ValueError):
         eng.train_step(x, y[:4])
     assert eng.micro_step == 0 and eng.comm.log == []
@@ -273,5 +219,5 @@ def test_micro_batches_of_a_channels_last_batch_stay_channels_last(cpu_engine):
             return self.net(x)
 
     eng = BnetDDP(Spy(), bucket_mb=0.002, comm=FakeComm(), accumulation_steps=3)
-    eng.train_step(*_batch(0))
+    eng.train_step(*batch(0, BATCH, 100))
     assert seen == [(4, True)] * 3

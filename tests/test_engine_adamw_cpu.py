@@ -7,40 +7,28 @@ import copy
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import HYPER, batch, close_params, make_pair, torch_step
 from engine_fakes import small_model as _model
 
 from bagua_net_b200.parallel.ddp import BnetDDP
-
-
-def _batch(step, channels_last=True):
-    torch.manual_seed(100 + step)
-    x, y = torch.randn(4, 3, 8, 8), torch.randint(0, 10, (4,))
-    return (x.contiguous(memory_format=torch.channels_last) if channels_last else x), y
-
-
-HYPER = dict(lr=3e-3, betas=(0.85, 0.99), eps=1e-7, weight_decay=0.05)
 
 
 @pytest.mark.parametrize("direct_grads", ["1", "0"], ids=["adopted", "accumulated"])
 @pytest.mark.parametrize("channels_last", [True, False])
 def test_engine_trains_like_torch_adamw(cpu_engine, channels_last, direct_grads):
     cpu_engine.setenv("BNET_DIRECT_GRADS", direct_grads)
-    ref, net = _model(channels_last), _model(channels_last)
-    opt = torch.optim.AdamW(ref.parameters(), **HYPER)
-    comm = FakeComm()
-    eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=comm, **HYPER)   # ~2 KB buckets: several of them
+    ref, opt, net, eng = make_pair("adamw", channels_last=channels_last, dtype=torch.float32)
+    comm = eng.comm
     assert len(eng.buckets) >= 2 and eng._hp is not None
     for step in range(6):
         if step == 3:                                          # a learning-rate schedule step mid-run
             eng.set_lr(1e-3, weight_decay=0.02)
             for g in opt.param_groups:
                 g["lr"], g["weight_decay"] = 1e-3, 0.02
-        x, y = _batch(step, channels_last)
-        opt.zero_grad()
-        l_ref = torch.nn.functional.cross_entropy(ref(x), y)
-        l_ref.backward()
-        l_ref = l_ref.detach()
-        opt.step()
+        x, y = batch(step, 4, 100, channels_last)
+        with torch.no_grad():
+            l_ref = torch.nn.functional.cross_entropy(ref(x), y)
+        torch_step(ref, opt, x, y)
         n0 = len(comm.steps_seen)
         l_eng = eng.train_step(x, y)
         # one fused launch per bucket, all reading this step's count; the count advances once per step
@@ -48,8 +36,7 @@ def test_engine_trains_like_torch_adamw(cpu_engine, channels_last, direct_grads)
         assert float(eng._hp[6]) == step + 1
         assert abs(float(l_eng) - float(l_ref)) < 1e-5, (step, float(l_eng), float(l_ref))
         assert float(eng.flat_grad.abs().max()) == 0.0
-    for a, b in zip(net.parameters(), ref.parameters()):
-        assert torch.allclose(a, b, rtol=0, atol=1e-5), (a - b).abs().max()
+    close_params(net, ref, 1e-5)
     for p in ref.parameters():                                 # (the engine's moments are torch's, shard by shard)
         assert opt.state[p]["step"] == 6
     assert eng.kernel_launches == 6 * len(eng.buckets)
@@ -58,22 +45,22 @@ def test_engine_trains_like_torch_adamw(cpu_engine, channels_last, direct_grads)
 def test_optimizer_state_round_trip_continues_bit_identically(cpu_engine):
     comm = FakeComm()
     net = _model()
-    eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=comm, **HYPER)
+    eng = BnetDDP(net, optimizer="adamw", bucket_mb=0.002, comm=comm, **HYPER["adamw"])
     for step in range(3):
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, 4, 100))
     weights = copy.deepcopy(net.state_dict())
     state = copy.deepcopy(eng.optimizer_state_dict())
-    assert state["optimizer"] == "adamw" and state["step"] == 3 and state["betas"] == HYPER["betas"]
-    assert state["eps"] == HYPER["eps"] and set(state["buckets"][0]) == {"master", "exp_avg", "exp_avg_sq"}
+    assert state["optimizer"] == "adamw" and state["step"] == 3 and state["betas"] == HYPER["adamw"]["betas"]
+    assert state["eps"] == HYPER["adamw"]["eps"] and set(state["buckets"][0]) == {"master", "exp_avg", "exp_avg_sq"}
     for step in range(3, 5):
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, 4, 100))
     fresh = _model()
     fresh.load_state_dict(weights)
     other = BnetDDP(fresh, optimizer="adamw", lr=0.5, betas=(0.5, 0.5), eps=1.0, bucket_mb=0.002, comm=FakeComm())
     other.load_optimizer_state_dict(state)
-    assert float(other._hp[6]) == 3.0 and other.betas == HYPER["betas"] and other.lr == HYPER["lr"]
+    assert float(other._hp[6]) == 3.0 and other.betas == HYPER["adamw"]["betas"] and other.lr == HYPER["adamw"]["lr"]
     for step in range(3, 5):
-        other.train_step(*_batch(step))
+        other.train_step(*batch(step, 4, 100))
     assert torch.equal(other.flat_param, eng.flat_param)
     for b1, b2 in zip(other.buckets, eng.buckets):
         for t1, t2 in zip(other._state(b1), eng._state(b2)):
@@ -105,7 +92,7 @@ def test_sgd_engine_is_unchanged(cpu_engine):
     comm = FakeComm()
     eng = BnetDDP(_model(), lr=0.1, weight_decay=1e-4, bucket_mb=0.002, comm=comm)
     assert eng.optimizer == "sgd" and eng.momentum == 0.9 and getattr(eng, "_hp", None) is None
-    eng.train_step(*_batch(0))
+    eng.train_step(*batch(0, 4, 100))
     assert comm.steps_seen == [] and comm.launches == len(eng.buckets)
     state = eng.optimizer_state_dict()
     assert set(state) == {"lr", "momentum", "weight_decay", "world", "rank", "buckets"}

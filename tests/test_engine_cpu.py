@@ -8,6 +8,7 @@ import copy
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import close_params, torch_step
 from engine_fakes import small_model as _model
 
 from bagua_net_b200.parallel import ddp as ddp_mod
@@ -48,17 +49,15 @@ def test_engine_trains_like_torch_sgd(cpu_engine, channels_last):
     if channels_last:
         x = x.contiguous(memory_format=torch.channels_last)
     for step in range(4):
-        opt.zero_grad()
-        l_ref = torch.nn.functional.cross_entropy(ref(x), y)
-        l_ref.backward()
-        opt.step()
+        with torch.no_grad():
+            l_ref = float(torch.nn.functional.cross_entropy(ref(x), y))
+        torch_step(ref, opt, x, y)
         n0 = comm.launches
         l_eng = eng.train_step(x, y)
         assert comm.launches - n0 == len(eng.buckets)           # one fused launch per bucket per step
-        assert abs(float(l_eng.detach()) - float(l_ref.detach())) < 1e-5, (step, float(l_eng.detach()), float(l_ref.detach()))
+        assert abs(float(l_eng.detach()) - l_ref) < 1e-5, (step, float(l_eng.detach()), l_ref)
         assert float(eng.flat_grad.abs().max()) == 0.0            # gradients are handed back zeroed
-    for a, b in zip(eng_model.parameters(), ref.parameters()):
-        assert torch.allclose(a, b, atol=1e-5), (a - b).abs().max()
+    close_params(eng_model, ref, 1e-5, rtol=1e-5)
     assert eng.kernel_launches == 4 * len(eng.buckets)
 
 
@@ -112,13 +111,10 @@ def test_producers_that_write_into_their_gradient_slice_are_adopted_without_a_co
         ref.load_state_dict(_DirectNet(direct=False).state_dict())
         opt = torch.optim.SGD(ref.parameters(), lr=lr, momentum=mom, weight_decay=wd)
         for _ in range(3):
-            opt.zero_grad()
-            torch.nn.functional.cross_entropy(ref(x), y).backward()
-            opt.step()
+            torch_step(ref, opt, x, y)
             eng.train_step(x, y)
             assert all(p.grad is None for p in net.parameters())          # nothing lingers between steps
-        for a, b in zip(net.parameters(), ref.parameters()):
-            assert torch.allclose(a, b, atol=1e-5), (direct, (a - b).abs().max())
+        close_params(net, ref, 1e-5, direct, rtol=1e-5)
         copies[direct] = eng.grad_copies
     # a registration dies with its owner (an engine lives as long as the model its hooks sit on; once both are gone the
     # buffers may be unmapped and the addresses reused)
@@ -171,8 +167,7 @@ def test_shared_weights_still_accumulate(cpu_engine):
         torch.nn.functional.cross_entropy(ref(x, direct=False), y).backward()
         opt.step()
         eng.train_step(x, y)
-    for a, b in zip(net.parameters(), ref.parameters()):
-        assert torch.allclose(a, b, atol=1e-5), (a - b).abs().max()
+    close_params(net, ref, 1e-5, rtol=1e-5)
 
 
 def test_engine_accumulate_mode_switch(cpu_engine):
@@ -184,13 +179,10 @@ def test_engine_accumulate_mode_switch(cpu_engine):
     assert all(p.grad is not None and p.grad.data_ptr() == eng._grad_view[id(p)].data_ptr() for p in net.parameters())
     x, y = torch.randn(4, 3, 8, 8).contiguous(memory_format=torch.channels_last), torch.randint(0, 10, (4,))
     for _ in range(3):
-        opt.zero_grad()
-        torch.nn.functional.cross_entropy(ref(x), y).backward()
-        opt.step()
+        torch_step(ref, opt, x, y)
         eng.train_step(x, y)
     assert eng.grad_copies == 0
-    for a, b in zip(net.parameters(), ref.parameters()):
-        assert torch.allclose(a, b, atol=1e-5)
+    close_params(net, ref, 1e-5, rtol=1e-5)
 
 
 def test_engine_lr_schedule_and_optimizer_state(cpu_engine):
@@ -273,13 +265,16 @@ def test_direct_grads_self_check_accepts_the_working_path_and_rejects_a_broken_o
 
 
 def test_fake_comm_takes_the_parameters_of_symm_comm():
-    """The CPU stand-in is called as the engine calls SymmComm: same parameter names, order and defaults."""
+    """The CPU stand-in is called as the engine calls SymmComm: every SymmComm method that ddp.py calls on its comm, with
+    the same parameter names, order and defaults."""
     import inspect
+    import re
 
     from bagua_net_b200.parallel.comm import SymmComm
 
-    for name in ("barrier", "fused_allreduce_sgd", "fused_allreduce_adamw", "fused_clip_reduce_norm", "fused_accum_reduce_norm",
-                 "fused_clip_coef", "fused_clip_apply_sgd", "fused_clip_apply_adamw", "lars_segments", "lars_tensors",
-                 "fused_lars_norm", "fused_lars_trust", "fused_lars_apply", "ema_update", "ema_advance"):
+    called = {n for n in re.findall(r"\bcomm\.(\w+)", inspect.getsource(ddp_mod)) if callable(getattr(SymmComm, n, None))}
+    world_above_one = {"peer_tensor", "broadcast_tensor"}      # only reached at world > 1; FakeComm is one rank
+    assert world_above_one < called
+    for name in sorted(called - world_above_one):
         want, got = (list(inspect.signature(getattr(c, name)).parameters.values()) for c in (SymmComm, FakeComm))
         assert [(p.name, p.default) for p in got] == [(p.name, p.default) for p in want], name

@@ -8,6 +8,7 @@ import copy
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import HYPER, LARC, Branchy, batch, make_pair, torch_step
 from engine_fakes import small_model as _model
 from torch.optim.swa_utils import AveragedModel, get_ema_multi_avg_fn
 
@@ -15,46 +16,7 @@ from bagua_net_b200.parallel.ddp import BnetDDP
 
 
 BATCH = 8
-HYPER = {"sgd": dict(lr=0.05, momentum=0.9, weight_decay=1e-3),
-         "adamw": dict(lr=3e-3, betas=(0.85, 0.99), eps=1e-7, weight_decay=0.05),
-         "lars": dict(lr=0.5, momentum=0.9, weight_decay=5e-4, trust_coefficient=0.02, eps=1e-8)}
 DECAY = 0.6                  # weights 0.4 (the lerp's first branch) and, after set_ema_decay(0.3), 0.7 (its second)
-
-
-def _batch(step):
-    torch.manual_seed(300 + step)
-    return torch.randn(BATCH, 3, 8, 8).contiguous(memory_format=torch.channels_last), torch.randint(0, 10, (BATCH,))
-
-
-def _engine(net, optimizer="sgd", **kw):
-    return BnetDDP(net, optimizer=optimizer, bucket_mb=0.002, comm=FakeComm(), **HYPER[optimizer], **kw)
-
-
-def _reference(ref, optimizer):
-    h = HYPER[optimizer]
-    if optimizer == "adamw":
-        return torch.optim.AdamW(ref.parameters(), **h)
-    return torch.optim.SGD(ref.parameters(), lr=h["lr"], momentum=h["momentum"],
-                           weight_decay=0.0 if optimizer == "lars" else h["weight_decay"])
-
-
-def _ref_step(ref, opt, optimizer, x, y, k, max_norm):
-    """One optimizer step of the float64 reference on the global batch (k micro-batches, clipped when max_norm)."""
-    opt.zero_grad()
-    for xs, ys in zip(x.split(BATCH // k), y.split(BATCH // k)):
-        (torch.nn.functional.cross_entropy(ref(xs.double()), ys) / k).backward()
-    if max_norm is not None:
-        torch.nn.utils.clip_grad_norm_(ref.parameters(), max_norm)
-    if optimizer == "lars":                               # Apex LARC(clip=False) in front of SGD
-        h = HYPER["lars"]
-        with torch.no_grad():
-            for p in ref.parameters():
-                if p.grad is None or p.dim() <= 1:
-                    continue
-                wn, gn = p.norm(), p.grad.norm()
-                if wn != 0 and gn != 0:
-                    p.grad.add_(p, alpha=h["weight_decay"]).mul_(h["trust_coefficient"] * wn / (gn + wn * h["weight_decay"] + h["eps"]))
-    opt.step()
 
 
 def _flat_ema(eng):
@@ -77,17 +39,15 @@ def _ema_f64(ema, master, decay, n):
 @pytest.mark.parametrize("optimizer", ["sgd", "adamw", "lars"])
 def test_ema_matches_averaged_model(cpu_engine, optimizer, clipped, every, k):
     thr = 0.05 if clipped else None
-    ref, net = _model().double(), _model()
-    opt = _reference(ref, optimizer)
+    ref, opt, net, eng = make_pair(optimizer, ema_decay=DECAY, ema_every=every, max_grad_norm=thr, accumulation_steps=k)
     avg = AveragedModel(ref, multi_avg_fn=get_ema_multi_avg_fn(DECAY), use_buffers=False)
-    eng = _engine(net, optimizer, ema_decay=DECAY, ema_every=every, max_grad_norm=thr, accumulation_steps=k)
     assert len(eng.buckets) >= 2
     assert torch.equal(_flat_ema(eng), torch.cat([b.master for b in eng.buckets]))   # a copy of the masters at first
     own = _flat_ema(eng).double()                          # float64 EMA of the engine's own masters
     n = 0
     for step in range(1, 8):
-        x, y = _batch(step)
-        _ref_step(ref, opt, optimizer, x, y, k, thr)
+        x, y = batch(step, BATCH, 300)
+        torch_step(ref, opt, x, y, k, max_norm=thr, lars=LARC if optimizer == "lars" else None)
         eng.train_step(x, y)
         if step % every == 0:
             avg.update_parameters(ref)
@@ -101,37 +61,23 @@ def test_ema_matches_averaged_model(cpu_engine, optimizer, clipped, every, k):
     assert int(avg.n_averaged) == n == 7 // every
 
 
-class _Branchy(torch.nn.Module):
-    def __init__(self, channels_last=True):
-        super().__init__()
-        torch.manual_seed(4)
-        self.unused = torch.nn.Linear(32, 32, bias=False)
-        self.net = _model(channels_last)
-
-    def forward(self, x):
-        return self.net(x)
-
-
 @pytest.mark.parametrize("optimizer", ["sgd", "lars"])
 def test_bucket_without_gradient_updates_its_ema(cpu_engine, optimizer):
-    net = _Branchy()
-    eng = _engine(net, optimizer, ema_decay=DECAY)
+    net, eng = make_pair(optimizer, model=Branchy, ema_decay=DECAY)[2:]
     idle = [b for b in eng.buckets if len(b.params) == 1 and b.params[0] is net.unused.weight]
     assert len(idle) == 1
     idle = idle[0]
-    eng.train_step(*_batch(0))                             # the copy step
+    eng.train_step(*batch(0, BATCH, 300))                  # the copy step
     assert torch.equal(idle.ema, idle.master)
     idle.ema.zero_()
-    eng.train_step(*_batch(1))                             # lerp(0, master, 0.4): the bucket's EMA moves without a gradient
+    eng.train_step(*batch(1, BATCH, 300))                  # lerp(0, master, 0.4): the bucket's EMA moves without a gradient
     assert torch.equal(idle.ema, torch.lerp(torch.zeros_like(idle.master), idle.master, float(eng._ema[0])))
     assert [kind for kind, _ in eng.comm.log].count("ema_update") == 2 * len(eng.buckets)
 
 
 def test_set_ema_decay_and_reset_ema_mid_run(cpu_engine):
-    ref, net = _model().double(), _model()
-    opt = _reference(ref, "sgd")
+    ref, opt, net, eng = make_pair("sgd", ema_decay=DECAY, ema_every=2)
     avg = AveragedModel(ref, multi_avg_fn=get_ema_multi_avg_fn(DECAY), use_buffers=False)
-    eng = _engine(net, ema_decay=DECAY, ema_every=2)
     for step in range(1, 11):
         if step == 4:                                      # a decay schedule: weight 0.7, the lerp's other branch
             eng.set_ema_decay(0.3)
@@ -139,8 +85,8 @@ def test_set_ema_decay_and_reset_ema_mid_run(cpu_engine):
         if step == 7:                                      # torchvision's n_averaged.fill_(0): the next update copies
             eng.reset_ema()
             avg.n_averaged.fill_(0)
-        x, y = _batch(step)
-        _ref_step(ref, opt, "sgd", x, y, 1, None)
+        x, y = batch(step, BATCH, 300)
+        torch_step(ref, opt, x, y)
         eng.train_step(x, y)
         if step % 2 == 0:
             avg.update_parameters(ref)
@@ -156,13 +102,13 @@ def test_set_ema_decay_and_reset_ema_mid_run(cpu_engine):
 @pytest.mark.parametrize("kind", ["sgd", "adamw", "lars", "sgd-clipped"])
 def test_launch_order(cpu_engine, kind, k):
     optimizer = kind.split("-")[0]
-    eng = _engine(_model(), optimizer, ema_decay=DECAY, ema_every=2, accumulation_steps=k,
-                  max_grad_norm=1.0 if "clipped" in kind else None)
+    eng = make_pair(optimizer, ema_decay=DECAY, ema_every=2, accumulation_steps=k,
+                    max_grad_norm=1.0 if "clipped" in kind else None)[3]
     nb, comm = len(eng.buckets), eng.comm
     update = "lars_apply" if optimizer == "lars" else "apply" if k > 1 or "clipped" in kind else optimizer
     for step in range(3):
         n0, l0 = len(comm.log), comm.launches
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, BATCH, 300))
         kinds = [kind for kind, _ in comm.log[n0:]]
         last = max(i for i, kd in enumerate(kinds) if kd == update)
         assert kinds.count(update) == nb                     # one optimizer step per train_step ...
@@ -175,10 +121,10 @@ def test_launch_order(cpu_engine, kind, k):
 def test_ema_parameters_publishes_and_restores(cpu_engine):
     for dtype in (torch.float32, torch.bfloat16):
         net = _model().to(dtype)
-        eng = _engine(net, ema_decay=DECAY, accumulation_steps=2)
+        eng = BnetDDP(net, bucket_mb=0.002, comm=FakeComm(), **HYPER["sgd"], ema_decay=DECAY, accumulation_steps=2)
         if dtype == torch.float32:
             for step in range(3):
-                eng.train_step(*_batch(step))
+                eng.train_step(*batch(step, BATCH, 300))
         torch.manual_seed(9)
         for b in eng.buckets:                              # an EMA away from the masters, below a bf16 ulp too
             b.ema.copy_(b.master + torch.randn_like(b.master) * 1e-3)
@@ -189,7 +135,7 @@ def test_ema_parameters_publishes_and_restores(cpu_engine):
             for p, e in zip(net.parameters(), _as_params(eng, net, _flat_ema(eng))):
                 assert torch.equal(p.detach(), e.to(dtype))
             with pytest.raises(ValueError):
-                eng.train_step(*_batch(0))
+                eng.train_step(*batch(0, BATCH, 300))
             with pytest.raises(ValueError):
                 eng.finish_step()
             with pytest.raises(ValueError):
@@ -197,7 +143,7 @@ def test_ema_parameters_publishes_and_restores(cpu_engine):
                     pass
         assert torch.equal(eng.flat_param.view(torch.uint8), before.view(torch.uint8))
         if dtype == torch.float32:                         # in the middle of an accumulation step
-            x, y = _batch(5)
+            x, y = batch(5, BATCH, 300)
             torch.nn.functional.cross_entropy(net(x[:4]), y[:4]).backward()
             eng.finish_step()
             assert eng.micro_step == 1
@@ -205,7 +151,7 @@ def test_ema_parameters_publishes_and_restores(cpu_engine):
                 with eng.ema_parameters():
                     pass
     with pytest.raises(ValueError):
-        with _engine(_model()).ema_parameters():
+        with make_pair("sgd")[3].ema_parameters():
             pass
 
 
@@ -215,15 +161,15 @@ EMA_KEYS = {"ema_decay", "ema_every", "ema_step", "ema_n_averaged"}
 
 @pytest.mark.parametrize("optimizer", ["sgd", "adamw", "lars"])
 def test_state_dict_round_trip(cpu_engine, optimizer):
-    eng = _engine(_model(), optimizer, ema_decay=DECAY, ema_every=2)
+    eng = make_pair(optimizer, ema_decay=DECAY, ema_every=2)[3]
     for step in range(5):
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, BATCH, 300))
     state = eng.optimizer_state_dict()
-    plain = set(_engine(_model(), optimizer).optimizer_state_dict())
+    plain = set(make_pair(optimizer)[3].optimizer_state_dict())
     assert set(state) == plain | EMA_KEYS
     assert (state["ema_decay"], state["ema_every"], state["ema_step"], state["ema_n_averaged"]) == (DECAY, 2, 5, 2)
     assert all("ema" in b and torch.equal(b["ema"], e.ema) for b, e in zip(state["buckets"], eng.buckets))
-    resumed = _engine(_model(), optimizer, ema_decay=0.9, ema_every=5)
+    resumed = make_pair(optimizer, ema_decay=0.9, ema_every=5)[3]
     resumed.load_optimizer_state_dict(copy.deepcopy(state))
     assert torch.equal(resumed._ema, eng._ema) and (resumed.ema_decay, resumed.ema_every) == (DECAY, 2)
     for b1, b2 in zip(resumed.buckets, eng.buckets):
@@ -231,18 +177,18 @@ def test_state_dict_round_trip(cpu_engine, optimizer):
 
 
 def test_state_dict_cross_loading(cpu_engine):
-    with_ema = _engine(_model(), ema_decay=DECAY)
-    without = _engine(_model())
+    with_ema = make_pair("sgd", ema_decay=DECAY)[3]
+    without = make_pair("sgd")[3]
     for step in range(2):
-        with_ema.train_step(*_batch(step))
-        without.train_step(*_batch(step))
+        with_ema.train_step(*batch(step, BATCH, 300))
+        without.train_step(*batch(step, BATCH, 300))
     # an EMA would be dropped silently: refused, and nothing is loaded
     masters = [b.master.clone() for b in without.buckets]
     with pytest.raises(ValueError):
         without.load_optimizer_state_dict(copy.deepcopy(with_ema.optimizer_state_dict()))
     assert all(torch.equal(m, b.master) for m, b in zip(masters, without.buckets))
     # a plain checkpoint into an engine with an EMA: the EMA restarts from the loaded masters
-    target = _engine(_model(), ema_decay=DECAY)
+    target = make_pair("sgd", ema_decay=DECAY)[3]
     target.load_optimizer_state_dict(copy.deepcopy(without.optimizer_state_dict()))
     for b, o in zip(target.buckets, without.buckets):
         assert torch.equal(b.master, o.master) and torch.equal(b.ema, o.master)
@@ -250,11 +196,11 @@ def test_state_dict_cross_loading(cpu_engine):
 
 
 def test_engine_without_ema_is_unchanged(cpu_engine):
-    eng = _engine(_model())
+    eng = make_pair("sgd")[3]
     assert eng.ema_decay is None and eng._ema is None and all(b.ema is None for b in eng.buckets)
     for step in range(2):
         n0, l0 = len(eng.comm.log), eng.comm.launches
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, BATCH, 300))
         assert [kind for kind, _ in eng.comm.log[n0:]] == ["sgd"] * len(eng.buckets)
         assert eng.comm.launches - l0 == len(eng.buckets)
     state = eng.optimizer_state_dict()
@@ -270,9 +216,9 @@ def test_rejects_bad_arguments(cpu_engine):
                 {"ema_decay": 0.9, "ema_every": -3}, {"ema_decay": 0.9, "ema_every": 2.0}, {"ema_decay": 0.9, "ema_every": True},
                 {"ema_decay": 0.9, "ema_every": "2"}, {"ema_decay": 0.9, "ema_every": (1 << 24) + 1}):
         with pytest.raises(ValueError):
-            _engine(_model(), **bad)
-    eng = _engine(_model(), ema_decay=0.0)               # the ends of [0, 1] are allowed
-    _engine(_model(), ema_decay=1, ema_every=1 << 24)
+            make_pair("sgd", **bad)
+    eng = make_pair("sgd", ema_decay=0.0)[3]               # the ends of [0, 1] are allowed
+    make_pair("sgd", ema_decay=1, ema_every=1 << 24)
     for bad in (-1e-9, 1.0000001, float("nan"), None):
         with pytest.raises(ValueError):
             eng.set_ema_decay(bad)

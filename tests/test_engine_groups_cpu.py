@@ -1,85 +1,18 @@
 """BnetDDP(param_groups=...)'s HOST logic on the CPU: every rejected argument, the group segment tables at world sizes 1-8
 on VGG16's and ResNet-50's real shapes, the device group table after set_lr / set_param_group / a state load, the
 state dict, and the engine against torch.optim.SGD / AdamW given the same groups (alone and with clipping, accumulation
-and the EMA).  GroupComm adds the grouped entry points to FakeComm as plain torch arithmetic per segment; the kernels
-are covered on the GPU by tests/test_param_groups.py."""
+and the EMA).  FakeComm does the grouped entry points as plain torch arithmetic per segment; the kernels are covered
+on the GPU by tests/test_param_groups.py."""
 import copy
 import math
 
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import batch, close_params, torch_step
 
 from bagua_net_b200.parallel.comm import GROUPS_MAX, check_group_segments
 from bagua_net_b200.parallel.ddp import BnetDDP, group_segments, no_weight_decay_groups, plan_buckets
-
-
-class GroupComm(FakeComm):
-    """FakeComm with the grouped steps: each segment of the validated table updated with its group's row."""
-
-    def __init__(self):
-        super().__init__()
-        self.tables = {}                   # id of an uploaded table -> (shard vectors, groups)
-
-    def group_segments(self, table, shard_vecs, ngroups):
-        check_group_segments(table, shard_vecs, ngroups)
-        t = torch.tensor(table, dtype=torch.int32).reshape(-1, 4)
-        self.tables[id(t)] = (shard_vecs, ngroups)
-        return t
-
-    def _per_segment(self, param, segs, groups, hp, update):
-        shard_vecs, ngroups = self.tables[id(segs)]
-        e = 16 // param.element_size()
-        assert shard_vecs * e == param.numel() and groups.shape == (groups.shape[0], 4) and groups.shape[0] >= ngroups
-        for vec0, nvec, g, _ in segs.tolist():
-            h = hp.clone()
-            h[0], h[4 if hp.numel() == 8 else 2] = groups[g, 0], groups[g, 1]
-            update(slice(vec0 * e, (vec0 + nvec) * e), h)
-
-    def _sgd_groups(self, g, param, master, mom, hp, groups, segs):
-        assert hp.numel() == 4
-        self._per_segment(param, segs, groups, hp, lambda s, h: self._sgd(g[s], param[s], master[s], mom[s], 0, 0, 0, None, h))
-        return float(hp[3])
-
-    def _adamw_groups(self, g, param, master, exp_avg, exp_avg_sq, hp, groups, segs):
-        steps = len(self.steps_seen)
-        self._per_segment(param, segs, groups, hp,
-                          lambda s, h: self._adamw(g[s], param[s], master[s], exp_avg[s], exp_avg_sq[s], h))
-        del self.steps_seen[steps + 1:]    # (one step, however many segments)
-        return float(hp[5])
-
-    def fused_allreduce_sgd_groups(self, grad, param, master, mom, hp, groups, segs, zero_grads=True, channel=0, nblocks=0,
-                                   stream=None):
-        self._sgd_groups(grad, param, master, mom, hp, groups, segs)
-        grad.zero_()
-        self._launched("sgd_groups", grad.numel())
-
-    def fused_allreduce_adamw_groups(self, grad, param, master, exp_avg, exp_avg_sq, hp, groups, segs, zero_grads=True,
-                                     channel=0, nblocks=0, stream=None):
-        self._adamw_groups(grad, param, master, exp_avg, exp_avg_sq, hp, groups, segs)
-        grad.zero_()
-        self._launched("adamw_groups", grad.numel())
-
-    def fused_clip_apply_sgd_groups(self, param, scratch, clip, master, mom, hp, groups, segs, channel=0, nblocks=0,
-                                    stream=None):
-        self.apply_scales.append(self._sgd_groups(scratch * clip[2], param, master, mom, hp, groups, segs))
-        self._launched("apply_groups", param.numel())
-
-    def fused_clip_apply_adamw_groups(self, param, scratch, clip, master, exp_avg, exp_avg_sq, hp, groups, segs, channel=0,
-                                      nblocks=0, stream=None):
-        self.apply_scales.append(self._adamw_groups(scratch * clip[2], param, master, exp_avg, exp_avg_sq, hp, groups, segs))
-        self._launched("apply_groups", param.numel())
-
-
-def test_group_comm_matches_symm_comm_signatures():
-    import inspect
-
-    from bagua_net_b200.parallel.comm import SymmComm
-
-    for name in ("group_segments", "fused_allreduce_sgd_groups", "fused_allreduce_adamw_groups", "fused_clip_apply_sgd_groups",
-                 "fused_clip_apply_adamw_groups"):
-        a, b = inspect.signature(getattr(GroupComm, name)), inspect.signature(getattr(SymmComm, name))
-        assert [(p.name, p.default) for p in a.parameters.values()] == [(p.name, p.default) for p in b.parameters.values()], name
 
 
 def _net():
@@ -122,16 +55,16 @@ def test_rejected_groups(cpu_engine):
     ]
     for groups, msg in cases:
         with pytest.raises(ValueError, match=msg):
-            BnetDDP(_net() if groups is None else net, comm=GroupComm(), param_groups=groups)
+            BnetDDP(_net() if groups is None else net, comm=FakeComm(), param_groups=groups)
     with pytest.raises(ValueError, match="not a trainable parameter"):
-        BnetDDP(frozen, comm=GroupComm(), param_groups=[{"params": [frozen[0].weight]}])
+        BnetDDP(frozen, comm=FakeComm(), param_groups=[{"params": [frozen[0].weight]}])
     with pytest.raises(ValueError, match="'sgd' and 'adamw'"):
-        BnetDDP(net, comm=GroupComm(), optimizer="lars", param_groups=[{"params": ps[:1]}])
+        BnetDDP(net, comm=FakeComm(), optimizer="lars", param_groups=[{"params": ps[:1]}])
     many = torch.nn.Sequential(*[torch.nn.Linear(2, 2, bias=False) for _ in range(GROUPS_MAX + 1)])
     mp = list(many.parameters())
     with pytest.raises(ValueError, match="at most 64"):      # 64 listed + the default group
-        BnetDDP(many, comm=GroupComm(), param_groups=[{"params": [p]} for p in mp[:GROUPS_MAX]])
-    eng = BnetDDP(many, comm=GroupComm(), param_groups=[{"params": [p]} for p in mp[:GROUPS_MAX - 1]])
+        BnetDDP(many, comm=FakeComm(), param_groups=[{"params": [p]} for p in mp[:GROUPS_MAX]])
+    eng = BnetDDP(many, comm=FakeComm(), param_groups=[{"params": [p]} for p in mp[:GROUPS_MAX - 1]])
     assert len(eng.param_groups) == GROUPS_MAX
     with pytest.raises(ValueError, match="not parameters of the module"):
         no_weight_decay_groups(net, names=["nope"])
@@ -139,7 +72,7 @@ def test_rejected_groups(cpu_engine):
 
 def test_set_param_group_rejects(cpu_engine):
     net = _net()
-    eng = BnetDDP(net, comm=GroupComm(), param_groups=_groups(net))
+    eng = BnetDDP(net, comm=FakeComm(), param_groups=_groups(net))
     for kw in ({"lr_scale": -1.0}, {"weight_decay": float("nan")}):
         with pytest.raises(ValueError):
             eng.set_param_group(0, **kw)
@@ -147,8 +80,8 @@ def test_set_param_group_rejects(cpu_engine):
         with pytest.raises(ValueError, match="does not exist"):
             eng.set_param_group(i, lr_scale=1.0)
     with pytest.raises(ValueError, match="no param groups"):
-        BnetDDP(_net(), comm=GroupComm()).set_param_group(0, lr_scale=1.0)
-    assert BnetDDP(_net(), comm=GroupComm()).param_groups is None
+        BnetDDP(_net(), comm=FakeComm()).set_param_group(0, lr_scale=1.0)
+    assert BnetDDP(_net(), comm=FakeComm()).param_groups is None
 
 
 # ------------------------------------------------------------------ the segment tables on real shapes
@@ -207,7 +140,7 @@ def _rows(eng):
 def test_device_table_follows_set_lr_set_param_group_and_load(cpu_engine):
     for optimizer in ("sgd", "adamw"):
         net = _net()
-        eng = BnetDDP(net, lr=0.1, weight_decay=1e-3, comm=GroupComm(), optimizer=optimizer, param_groups=_groups(net))
+        eng = BnetDDP(net, lr=0.1, weight_decay=1e-3, comm=FakeComm(), optimizer=optimizer, param_groups=_groups(net))
         assert [g["lr_scale"] for g in eng.param_groups] == [1.0, 10.0, 1.0]
         assert [g["weight_decay"] for g in eng.param_groups] == [0.0, 1e-3, 1e-3]
         assert sum(len(g["params"]) for g in eng.param_groups) == len(list(net.parameters()))
@@ -225,16 +158,16 @@ def test_device_table_follows_set_lr_set_param_group_and_load(cpu_engine):
         assert sd["param_groups"][1] == {"params": sd["param_groups"][1]["params"], "lr_scale": 0.5, "weight_decay": None}
         assert sd["param_groups"][2]["weight_decay"] == 0.0
         net2 = _net()
-        eng2 = BnetDDP(net2, lr=1.0, comm=GroupComm(), optimizer=optimizer, param_groups=_groups(net2))
+        eng2 = BnetDDP(net2, lr=1.0, comm=FakeComm(), optimizer=optimizer, param_groups=_groups(net2))
         eng2.load_optimizer_state_dict(copy.deepcopy(sd))
         assert eng2.lr == 0.03 and eng2._groups.tolist() == eng._groups.tolist()
         assert eng2.optimizer_state_dict()["param_groups"] == sd["param_groups"]
         # membership differs; groups on one side only
         net3 = _net()
-        eng3 = BnetDDP(net3, comm=GroupComm(), optimizer=optimizer, param_groups=no_weight_decay_groups(net3))
+        eng3 = BnetDDP(net3, comm=FakeComm(), optimizer=optimizer, param_groups=no_weight_decay_groups(net3))
         with pytest.raises(ValueError, match="other parameters"):
             eng3.load_optimizer_state_dict(copy.deepcopy(sd))
-        plain = BnetDDP(_net(), comm=GroupComm(), optimizer=optimizer)
+        plain = BnetDDP(_net(), comm=FakeComm(), optimizer=optimizer)
         with pytest.raises(ValueError, match="disagree on param groups"):
             plain.load_optimizer_state_dict(copy.deepcopy(sd))
         with pytest.raises(ValueError, match="disagree on param groups"):
@@ -243,7 +176,7 @@ def test_device_table_follows_set_lr_set_param_group_and_load(cpu_engine):
 
 
 def test_ungrouped_engine_is_unchanged(cpu_engine):
-    comm = GroupComm()
+    comm = FakeComm()
     eng = BnetDDP(_net(), comm=comm)
     assert eng._hp is None and eng._groups is None and all(b.gsegs is None for b in eng.buckets)
     x, y = torch.randn(4, 3, 8, 8), torch.randint(0, 10, (4,))
@@ -269,7 +202,7 @@ def test_engine_matches_torch_optim_with_groups(cpu_engine, optimizer, extra):
     hyper = dict(lr=0.05, momentum=0.9, weight_decay=1e-2) if optimizer == "sgd" else dict(lr=2e-3, betas=(0.9, 0.99), eps=1e-8,
                                                                                             weight_decay=0.05)
     net, ref = _net().eval(), _net().double().eval()          # (eval: BatchNorm statistics need no accumulation rule)
-    comm = GroupComm()
+    comm = FakeComm()
     eng = BnetDDP(net, comm=comm, optimizer=optimizer, bucket_mb=0.002, param_groups=_groups(net), **hyper, **extra)
     assert len(eng.buckets) > 1
     k = extra.get("accumulation_steps", 1)
@@ -285,23 +218,16 @@ def test_engine_matches_torch_optim_with_groups(cpu_engine, optimizer, extra):
             eng.set_param_group(1, lr_scale=3.0)
             for g, (glr, gwd) in zip(opt.param_groups, [(lr, 0.0), (lr * 3.0, wd), (lr, wd)]):
                 g["lr"], g["weight_decay"] = glr, gwd
-        torch.manual_seed(100 + step)
-        x, y = torch.randn(8, 3, 8, 8), torch.randint(0, 10, (8,))
+        x, y = batch(step, 8, 100, channels_last=False)
         eng.train_step(x, y)
-        opt.zero_grad()
-        for xs, ys in zip(x.split(8 // k), y.split(8 // k)):
-            (torch.nn.functional.cross_entropy(ref(xs.double()), ys) / k).backward()
-        if "max_grad_norm" in extra:
-            torch.nn.utils.clip_grad_norm_(ref.parameters(), extra["max_grad_norm"])
-        opt.step()
+        torch_step(ref, opt, x, y, k, max_norm=extra.get("max_grad_norm"))
         if "ema_decay" in extra:
             with torch.no_grad():
                 for e, p in zip(ema, ref.parameters()):
                     e.copy_(p if step == 0 else torch.lerp(e, p, 0.5))
     kinds = {kind for kind, _ in comm.log}
     assert ("apply_groups" if eng._staged else f"{optimizer}_groups") in kinds and not kinds & {"sgd", "adamw", "apply"}
-    for p, r in zip(net.parameters(), ref.parameters()):
-        assert torch.allclose(p.double(), r, rtol=1e-4, atol=1e-5), (optimizer, extra)
+    close_params(net, ref, 1e-5, (optimizer, extra), rtol=1e-4)
     if "ema_decay" in extra:
         with eng.ema_parameters():
             for p, e in zip(net.parameters(), ema):
@@ -310,8 +236,8 @@ def test_engine_matches_torch_optim_with_groups(cpu_engine, optimizer, extra):
 
 def test_groups_do_not_change_buckets_or_state_layout(cpu_engine):
     net_a, net_b = _net(), _net()
-    a = BnetDDP(net_a, comm=GroupComm(), bucket_mb=0.002)
-    b = BnetDDP(net_b, comm=GroupComm(), bucket_mb=0.002, param_groups=_groups(net_b))
+    a = BnetDDP(net_a, comm=FakeComm(), bucket_mb=0.002)
+    b = BnetDDP(net_b, comm=FakeComm(), bucket_mb=0.002, param_groups=_groups(net_b))
     assert [(x.start, x.numel, len(x.params)) for x in a.buckets] == [(x.start, x.numel, len(x.params)) for x in b.buckets]
     assert [t.shape for x in a.buckets for t in x.state] == [t.shape for x in b.buckets for t in x.state]
     assert math.isclose(b.param_groups[1]["lr"], 0.1)

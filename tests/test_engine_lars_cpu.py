@@ -9,6 +9,7 @@ import math
 import pytest
 import torch
 from engine_fakes import FakeComm, cpu_engine  # noqa: F401 - cpu_engine is a fixture
+from engine_fakes import LARC, Branchy, batch, close_params, make_pair, torch_step
 from engine_fakes import small_model as _model
 
 from bagua_net_b200.parallel.comm import LARS_CHUNK, check_lars_segments, check_lars_tensors
@@ -79,46 +80,7 @@ def test_padding_only_shard_and_rejected_tables():
 
 
 # ------------------------------------------------------------------ the engine against float64 LARC + SGD
-LARS = dict(lr=0.5, momentum=0.9, weight_decay=5e-4, trust_coefficient=0.02, eps=1e-8)
 BATCH = 8
-
-
-def _batch(step, channels_last=True):
-    torch.manual_seed(200 + step)
-    x, y = torch.randn(BATCH, 3, 8, 8), torch.randint(0, 10, (BATCH,))
-    return (x.contiguous(memory_format=torch.channels_last) if channels_last else x), y
-
-
-def larc_step(params, opt, wd, eta, eps):
-    """NVIDIA Apex LARC(clip=False) on the .grad of `params` (float64), then `opt` (torch.optim.SGD, weight_decay=0)."""
-    with torch.no_grad():
-        for p in params:
-            if p.grad is None or p.dim() <= 1:
-                continue
-            wn, gn = p.norm(), p.grad.norm()
-            if wn != 0 and gn != 0:
-                t = eta * wn / (gn + wn * wd + eps)
-                p.grad.add_(p, alpha=wd).mul_(t)
-    opt.step()
-
-
-def _pair(channels_last=True, model=None, **kw):
-    make = model or _model
-    ref, net = make(channels_last).double(), make(channels_last)
-    opt = torch.optim.SGD(ref.parameters(), lr=LARS["lr"], momentum=LARS["momentum"])
-    eng = BnetDDP(net, optimizer="lars", bucket_mb=0.002, comm=FakeComm(), **LARS, **kw)
-    return ref, opt, net, eng
-
-
-def _ref_step(ref, opt, x, y, k, max_norm, lr):
-    for g in opt.param_groups:
-        g["lr"] = lr
-    opt.zero_grad()
-    for xs, ys in zip(x.split(BATCH // k), y.split(BATCH // k)):
-        (torch.nn.functional.cross_entropy(ref(xs.double()), ys) / k).backward()
-    norm = torch.nn.utils.clip_grad_norm_(ref.parameters(), max_norm if max_norm is not None else math.inf)
-    larc_step(list(ref.parameters()), opt, LARS["weight_decay"], LARS["trust_coefficient"], LARS["eps"])
-    return float(norm)
 
 
 @pytest.mark.parametrize("k", [1, 2])
@@ -128,36 +90,35 @@ def _ref_step(ref, opt, x, y, k, max_norm, lr):
 def test_lars_engine_trains_like_larc_and_sgd(cpu_engine, k, clipped, direct_grads, channels_last):
     cpu_engine.setenv("BNET_DIRECT_GRADS", direct_grads)
     thr = 0.05 if clipped else None
-    ref, opt, net, eng = _pair(channels_last, max_grad_norm=thr, accumulation_steps=k)
+    ref, opt, net, eng = make_pair("lars", channels_last=channels_last, max_grad_norm=thr, accumulation_steps=k)
     assert len(eng.buckets) >= 2 and eng._staged
-    lr = LARS["lr"]
     for step in range(4):
         if step == 2:
-            lr = 0.2
-            eng.set_lr(lr)                                          # mid-run: the device block, no re-capture
-        x, y = _batch(step, channels_last)
-        want = _ref_step(ref, opt, x, y, k, thr, lr)
+            eng.set_lr(0.2)                                         # mid-run: the device block, no re-capture
+            for g in opt.param_groups:
+                g["lr"] = 0.2
+        x, y = batch(step, BATCH, 200, channels_last)
+        want = torch_step(ref, opt, x, y, k, max_norm=thr, lars=LARC)
         eng.train_step(x, y)
         if clipped:
             assert float(eng.last_grad_norm) == pytest.approx(want, rel=1e-5)
         assert float(eng.flat_grad.abs().max()) == 0.0
-        for a, b in zip(net.parameters(), ref.parameters()):
-            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5), (step, float((a.double() - b).abs().max()))
+        close_params(net, ref, 2e-5, step)
         t = eng.last_trust_ratios
         assert t.shape == (len(list(net.parameters())),) and t.dtype == torch.float32
         for ti, p in zip(t.tolist(), net.parameters()):
             assert (ti == 1.0) if p.dim() <= 1 else (0.0 < ti < math.inf and ti != 1.0)
-    assert float(eng._hp[0]) == pytest.approx(0.2) and float(eng._hp[4]) == pytest.approx(LARS["trust_coefficient"])
+    assert float(eng._hp[0]) == pytest.approx(0.2) and float(eng._hp[4]) == pytest.approx(LARC["trust_coefficient"])
 
 
 @pytest.mark.parametrize("clipped", [False, True], ids=["unclipped", "clipped"])
 @pytest.mark.parametrize("k", [1, 2])
 def test_launch_order(cpu_engine, clipped, k):
-    ref, opt, net, eng = _pair(max_grad_norm=1.0 if clipped else None, accumulation_steps=k)
+    eng = make_pair("lars", max_grad_norm=1.0 if clipped else None, accumulation_steps=k)[3]
     nb, comm = len(eng.buckets), eng.comm
     for step in range(2):
         n0, l0 = len(comm.log), comm.launches
-        eng.train_step(*_batch(step))
+        eng.train_step(*batch(step, BATCH, 200))
         kinds = [kind for kind, _ in comm.log[n0:]]
         want = ["norm"] * nb + ["accum"] * nb * (k - 1) + (["coef"] if clipped else [])
         want += ["lars_norm"] * nb + ["lars_trust"] + ["lars_apply"] * nb
@@ -172,42 +133,30 @@ def test_other_optimizers_have_no_trust_ratios(cpu_engine):
         assert eng.last_trust_ratios is None
 
 
-class _Branchy(torch.nn.Module):
-    def __init__(self, channels_last=True):
-        super().__init__()
-        torch.manual_seed(4)
-        self.unused = torch.nn.Linear(32, 32, bias=False)
-        self.net = _model(channels_last)
-
-    def forward(self, x):
-        return self.net(x)
-
-
 def test_bucket_without_gradient_is_left_alone(cpu_engine):
-    ref, opt, net, eng = _pair(model=_Branchy)
+    ref, opt, net, eng = make_pair("lars", model=Branchy)
     idle = [k for k, b in enumerate(eng.buckets) if len(b.params) == 1 and b.params[0] is net.unused.weight]
     assert len(idle) == 1
     w0 = net.unused.weight.detach().clone()
     eng._lars_slots.fill_(7.0)                                       # stale sums must not reach the ratios
     for step in range(2):
-        x, y = _batch(step)
+        x, y = batch(step, BATCH, 200)
         ref.unused.weight.grad = None
-        _ref_step(ref, opt, x, y, 1, None, LARS["lr"])
+        torch_step(ref, opt, x, y, lars=LARC)
         eng.train_step(x, y)
-        for a, b in zip(net.parameters(), ref.parameters()):
-            assert torch.allclose(a.double(), b, rtol=0, atol=2e-5)
+        close_params(net, ref, 2e-5, step)
     assert torch.equal(net.unused.weight, w0)
     assert float(eng.last_trust_ratios[0]) == 1.0                    # (`unused` is the first parameter)
     assert [kind for kind, _ in eng.comm.log].count("lars_apply") == 2 * (len(eng.buckets) - 1)
 
 
 def test_state_dict_round_trip_and_keys(cpu_engine):
-    ref, opt, net, eng = _pair()
-    eng.train_step(*_batch(0))
+    eng = make_pair("lars")[3]
+    eng.train_step(*batch(0, BATCH, 200))
     state = eng.optimizer_state_dict()
     assert set(state) == {"optimizer", "lr", "momentum", "weight_decay", "trust_coefficient", "eps", "world", "rank", "buckets"}
     assert state["optimizer"] == "lars" and all(set(b) == {"master", "momentum"} for b in state["buckets"])
-    resumed = _pair()[3]
+    resumed = make_pair("lars")[3]
     resumed.load_optimizer_state_dict(copy.deepcopy(state))
     for b1, b2 in zip(resumed.buckets, eng.buckets):
         assert all(torch.equal(t1, t2) for t1, t2 in zip(b1.state, b2.state))
