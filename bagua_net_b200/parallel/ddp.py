@@ -183,6 +183,49 @@ def group_segments(members, numels, group_of, start: int, numel: int, element_si
     return rows
 
 
+# ------------------------------------------------------------------ the shard <-> full mapping of the optimizer state
+def shard_pieces(plan, numels, world: int, rank: int) -> list:
+    """Where every bucket's shard on one rank comes from: per bucket of ``plan`` (plan_buckets), the pieces
+    ``(parameter index, first element in the parameter, count, offset in the shard)`` in shard order.  Elements are
+    counted in the parameter's memory order (as the flat buffer holds it: ``memory_flat``).  Shard elements that no piece
+    covers are padding (the 16-byte alignment after a tensor, the bucket quantum at its end), and a shard may hold no
+    piece at all."""
+    out = []
+    for start, numel, members in plan:
+        shard = numel // world
+        lo, hi = start + rank * shard, start + (rank + 1) * shard
+        pieces = []
+        for pi, off in members:
+            a, b = max(off, lo), min(off + numels[pi], hi)
+            if a < b:
+                pieces.append((pi, a - off, b - a, a - lo))
+        out.append(pieces)
+    return out
+
+
+def shard_from_full(flats, pieces, shard: torch.Tensor) -> torch.Tensor:
+    """Fill one bucket's ``shard`` from ``flats`` (every parameter's values, flat in memory order) along ``pieces`` (one
+    bucket's entry of ``shard_pieces``); the padding becomes zero.  Returns ``shard``."""
+    shard.zero_()
+    for pi, p0, n, s0 in pieces:
+        shard[s0:s0 + n].copy_(flats[pi][p0:p0 + n])
+    return shard
+
+
+def full_from_shard(flats, pieces, shard: torch.Tensor) -> None:
+    """The inverse of ``shard_from_full``: copy the pieces of one bucket's ``shard`` into ``flats``; padding is dropped."""
+    for pi, p0, n, s0 in pieces:
+        flats[pi][p0:p0 + n].copy_(shard[s0:s0 + n])
+
+
+def memory_flat(t: torch.Tensor) -> torch.Tensor:
+    """A 1-D view of ``t`` in the element order the flat buffers use for a parameter of its layout: NHWC for a
+    channels_last 4-D tensor (as BnetDDP keeps such filters), the logical order for a contiguous one."""
+    if t.dim() == 4 and not t.is_contiguous() and t.is_contiguous(memory_format=torch.channels_last):
+        return t.permute(0, 2, 3, 1).view(-1)
+    return t.view(-1)
+
+
 def no_weight_decay_groups(module: torch.nn.Module, names=()) -> list:
     """The usual param group without weight decay: ``[{"params": [...], "weight_decay": 0.0}]`` with every trainable
     parameter of ``module`` that has ``p.dim() <= 1`` (biases, normalisation weights) or whose name (as in
@@ -245,6 +288,17 @@ def _parse_param_groups(param_groups, params):
     if len(scales) > GROUPS_MAX:
         raise ValueError(f"{len(scales)} param groups (the default group included): the kernels take at most {GROUPS_MAX}")
     return group_of, scales, wds
+
+
+def _torch_optimizer_kind(groups) -> str:
+    """"adamw" or "sgd" for the param groups of a torch.optim.AdamW / SGD state_dict(); ValueError for anything else."""
+    g = groups[0] if groups else {}
+    if "betas" in g and "amsgrad" in g and g.get("decoupled_weight_decay", True):
+        return "adamw"
+    if "momentum" in g and "dampening" in g and "nesterov" in g:
+        return "sgd"
+    raise ValueError(f"not a torch.optim.SGD or AdamW state (param group keys {sorted(g)}); the engine fuses SGD, AdamW "
+                     "and LARS")
 
 
 def _check_max_norm(v) -> float:
@@ -382,11 +436,12 @@ class BnetDDP(torch.nn.Module):
             if optimizer == "lars":
                 raise ValueError("param_groups are offered for 'sgd' and 'adamw'; LARS excludes p.dim() <= 1 tensors itself")
             self._group_of, self._group_scale, self._group_wd = _parse_param_groups(param_groups, params)
-            self._params = params
+        self._params = params
         self.dtype = dtype
         es = params[0].element_size()
         world = dist.get_world_size(group) if dist.is_initialized() else 1
         plan, total = plan_buckets([p.numel() for p in params], es, world, bucket_mb)
+        self._plan = plan                # (the full optimizer state dict maps shards to parameters through it)
         self.buckets: list[_Bucket] = []
         layout = []
         for start, numel, members in plan:
@@ -967,7 +1022,8 @@ class BnetDDP(torch.nn.Module):
                 raise ValueError("the optimizer state's param groups hold other parameters than this engine's")
             scales = [_check_group_value("lr_scale", g["lr_scale"]) for g in groups]
             wds = [None if g["weight_decay"] is None else _check_group_value("weight_decay", g["weight_decay"]) for g in groups]
-            self._group_scale, self._group_wd = scales, wds
+        else:
+            scales = wds = None
         for b, s in zip(self.buckets, state["buckets"]):
             for k, t in zip(_STATE_NAMES[self.optimizer], b.state):
                 t.copy_(s[k])
@@ -979,20 +1035,225 @@ class BnetDDP(torch.nn.Module):
                 b.ema.copy_(s["ema"] if has_ema else b.master)
             counts = (state["ema_step"], state["ema_n_averaged"]) if has_ema else (0, 0)
             self._ema.copy_(torch.tensor(self._ema_block(*counts), dtype=torch.float32))
+        self._restore_hyper(state["lr"], state["weight_decay"], state, scales, wds, state.get("step", 0))
+
+    # The layout-free format: torch.optim.Optimizer.state_dict()'s layout, with no trace of the world size, the rank or the
+    # buckets, plus a "bnet" entry for what torch has no slot for.  Index i numbers the trainable parameters group by
+    # group in the order of `param_groups` (default group last), module order within a group: the numbering torch.optim
+    # gives when it is built from those groups.
+    _FULL_VERSION = 1
+    _TORCH_STATE = {"sgd": ("momentum_buffer",), "lars": ("momentum_buffer",), "adamw": ("exp_avg", "exp_avg_sq")}
+
+    def _check_checkpoint_call(self, what: str) -> None:
+        self._check_step_boundary(what)
+        if self._in_ema:
+            raise ValueError(f"cannot {what} inside ema_parameters(): the parameters hold the EMA weights")
+        if self.flat_param.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise ValueError(f"cannot {what} inside a CUDA graph capture")
+
+    def _torch_order(self) -> list:
+        """The engine's parameter index (module order) of every torch.optim index."""
+        if self._groups is None:
+            return list(range(len(self._params)))
+        return [j for k in range(len(self._group_scale)) for j, g in enumerate(self._group_of) if g == k]
+
+    def _torch_groups(self) -> list:
+        """torch.optim's param groups with the effective values, each with its ``lr_scale``, ``params`` as torch indices."""
         if self.optimizer == "adamw":
-            self.lr, self.weight_decay, self.eps = state["lr"], state["weight_decay"], state["eps"]
-            self.betas = tuple(state["betas"])
-            self._hp.copy_(torch.tensor(self._adamw_hp(state["step"]), dtype=torch.float32))
+            hyper = {"betas": tuple(self.betas), "eps": self.eps, "amsgrad": False, "maximize": False,
+                     "decoupled_weight_decay": True}     # (without it torch.optim.AdamW.load_state_dict turns into Adam)
+        else:
+            hyper = {"momentum": self.momentum, "dampening": 0, "nesterov": False, "maximize": False}
+            if self.optimizer == "lars":
+                hyper.update(trust_coefficient=self.trust_coefficient, eps=self.eps)
+        if self._groups is None:
+            groups = [(len(self._params), 1.0, self.weight_decay)]
+        else:
+            groups = [(self._group_of.count(k), s, self.weight_decay if wd is None else wd)
+                      for k, (s, wd) in enumerate(zip(self._group_scale, self._group_wd))]
+        out, i = [], 0
+        for n, s, wd in groups:
+            out.append({"lr": self.lr * s, **hyper, "weight_decay": wd, "lr_scale": s, "params": list(range(i, i + n))})
+            i += n
+        return out
+
+    def full_optimizer_state_dict(self) -> dict | None:
+        """The whole optimizer state, independent of the world size and the bucket layout, in the layout of
+        ``torch.optim.Optimizer.state_dict()`` (see docs/API.md).  Collective: every rank calls it; rank 0 gets the dict
+        (tensors in host memory), the other ranks ``None``.  The shards travel bucket by bucket, one source rank at a
+        time, through the heap's broadcast, so no rank holds more than one shard of one bucket on the device."""
+        self._check_checkpoint_call("save the optimizer state")
+        world, rank = self.comm.world, self.comm.rank
+        names = _STATE_NAMES[self.optimizer] + (("ema",) if self._ema is not None else ())
+        step = int(self._hp[self._HP_STEP].item()) if self.optimizer == "adamw" else None
+        counts = [int(v) for v in self._ema[self._EMA_STEP:].tolist()] if self._ema is not None else None
+        fulls = flats = pieces = None
+        if rank == 0:
+            fulls = {n: [torch.empty_like(p, dtype=torch.float32, device="cpu") for p in self._params] for n in names}
+            flats = {n: [memory_flat(t) for t in ts] for n, ts in fulls.items()}
+            numels = [p.numel() for p in self._params]
+            pieces = [shard_pieces(self._plan, numels, world, r) for r in range(world)]
+        for k, b in enumerate(self.buckets):
+            for n, t in zip(names, b.state + ((b.ema,) if b.ema is not None else ())):
+                for src in range(world):
+                    shard = t.detach()
+                    if src != 0:                  # (collective: every rank takes part in every source's broadcast)
+                        shard = shard.clone() if rank == src else torch.empty_like(t)
+                        self.comm.broadcast_tensor(shard, src=src)
+                    if rank == 0:                 # (each piece straight from the device into its host tensor)
+                        full_from_shard(flats[n], pieces[src][k], shard)
+        if rank != 0:
+            return None
+        order = self._torch_order()
+        if self.optimizer == "adamw":
+            state = {i: {"step": torch.tensor(float(step), dtype=torch.float32), "exp_avg": fulls["exp_avg"][j],
+                         "exp_avg_sq": fulls["exp_avg_sq"][j]} for i, j in enumerate(order)}
+        else:
+            state = {i: {"momentum_buffer": fulls["momentum"][j]} for i, j in enumerate(order)}
+        bnet = {"version": self._FULL_VERSION, "optimizer": self.optimizer, "lr": self.lr, "weight_decay": self.weight_decay,
+                "group_weight_decay": None if self._groups is None else list(self._group_wd),
+                "master": {i: fulls["master"][j] for i, j in enumerate(order)}}
+        if step is not None:
+            bnet["step"] = step
+        if self._ema is not None:
+            bnet.update(ema={i: fulls["ema"][j] for i, j in enumerate(order)}, ema_decay=self.ema_decay,
+                        ema_every=self.ema_every, ema_step=counts[0], ema_n_averaged=counts[1])
+        return {"state": state, "param_groups": self._torch_groups(), "bnet": bnet}
+
+    def load_full_optimizer_state_dict(self, state: dict) -> None:
+        """Load a dict of ``full_optimizer_state_dict`` (saved at any world size and ``bucket_mb``), or a plain
+        ``torch.optim.SGD`` / ``AdamW`` ``state_dict()``.  Every rank calls it with the same dict and copies out its own
+        shards; no communication.  Raises ValueError for a state the engine cannot represent (see docs/API.md)."""
+        self._check_checkpoint_call("load an optimizer state")
+        groups = list(state["param_groups"])
+        bnet = state.get("bnet")
+        ours = self._torch_groups()
+        if bnet is None:
+            kind = _torch_optimizer_kind(groups)
+            if kind != self.optimizer:
+                raise ValueError(f"a torch.optim {kind} state cannot be loaded into a {self.optimizer!r} engine")
+            if self._groups is None and len(groups) > 1:
+                raise ValueError(f"the torch.optim state has {len(groups)} param groups and this engine none: build it "
+                                 "with the same param_groups")
+        else:
+            if bnet.get("version") != self._FULL_VERSION:
+                raise ValueError(f"unknown full optimizer state version {bnet.get('version')!r}")
+            kind = bnet["optimizer"]
+            if kind != self.optimizer:
+                raise ValueError(f"optimizer state of {kind!r} cannot be loaded into a {self.optimizer!r} engine")
+            if (bnet["group_weight_decay"] is None) != (self._groups is None):
+                raise ValueError("the optimizer state and this engine disagree on param groups: one has them, the other not")
+            if "ema" in bnet and self._ema is None:
+                raise ValueError("the optimizer state holds an EMA of the weights, which this engine would drop: build it "
+                                 "with ema_decay=... to load it")
+        if [list(g["params"]) for g in groups] != [g["params"] for g in ours]:
+            raise ValueError("the optimizer state's param groups hold other parameters than this engine's")
+        order = self._torch_order()
+        per_param = state.get("state", {})
+        values = {n: [None] * len(order) for n in self._TORCH_STATE[self.optimizer]}
+        steps = set()
+        for i, j in enumerate(order):
+            entry = per_param.get(i) or {}
+            for n in values:
+                v = entry.get(n)
+                if v is not None:
+                    values[n][j] = self._check_full_shape(v, j, n)
+            if self.optimizer == "adamw" and entry.get("step") is not None:
+                steps.add(float(entry["step"]))
+        if bnet is None:
+            lr, wd, step, scales, wds = self._torch_hyper(groups, steps)
+            master = ema = None
+        else:
+            lr, wd, step = bnet["lr"], bnet["weight_decay"], bnet.get("step", 0)
+            scales = [_check_group_value("lr_scale", g["lr_scale"]) for g in groups]
+            wds = [None if v is None else _check_group_value("weight_decay", v) for v in bnet["group_weight_decay"] or ()]
+            master, ema = [None] * len(order), [None] * len(order) if "ema" in bnet else None
+            for i, j in enumerate(order):
+                master[j] = self._check_full_shape(bnet["master"][i], j, "master")
+                if ema is not None:
+                    ema[j] = self._check_full_shape(bnet["ema"][i], j, "ema")
+        # everything is checked: from here on nothing raises
+        numels = [p.numel() for p in self._params]
+        for b, pieces in zip(self.buckets, shard_pieces(self._plan, numels, self.comm.world, self.comm.rank)):
+            srcs = [master] + [values[n] for n in self._TORCH_STATE[self.optimizer]]
+            if self._ema is not None:
+                srcs.append(ema)
+            for t, src in zip(b.state + ((b.ema,) if b.ema is not None else ()), srcs):
+                if src is None:
+                    continue                      # (masters from the parameters, an EMA from the masters: below)
+                shard_from_full({pi: self._layout_flat(src[pi], pi) for pi, _, _, _ in pieces}, pieces, t)
+        if master is None:
+            self.sync_master_from_params()
+        if self._ema is not None:
+            counts = (0, 0)
+            if ema is not None:
+                self.ema_decay, self.ema_every = _check_ema_decay(bnet["ema_decay"]), int(bnet["ema_every"])
+                counts = (bnet["ema_step"], bnet["ema_n_averaged"])
+            else:
+                for b in self.buckets:
+                    b.ema.copy_(b.master)
+            self._ema.copy_(torch.tensor(self._ema_block(*counts), dtype=torch.float32))
+        self._restore_hyper(lr, wd, groups[-1], scales, wds, step)
+
+    def _check_full_shape(self, v, j: int, what: str) -> torch.Tensor:
+        p = self._params[j]
+        if not isinstance(v, torch.Tensor) or tuple(v.shape) != tuple(p.shape):
+            raise ValueError(f"the optimizer state's {what} of parameter {j} has shape "
+                             f"{tuple(v.shape) if isinstance(v, torch.Tensor) else type(v).__name__}, the parameter "
+                             f"{tuple(p.shape)}")
+        return v
+
+    def _layout_flat(self, v, pi: int) -> torch.Tensor:
+        """``v`` (parameter ``pi``'s shape, any layout and device; None: zeros) as fp32 in the parameter's memory order."""
+        p = self._params[pi]
+        if v is None:
+            return torch.zeros(p.numel(), dtype=torch.float32)
+        if v.dtype != torch.float32 or v.stride() != p.stride():
+            v = torch.empty_like(p, dtype=torch.float32, device=v.device).copy_(v)
+        return memory_flat(v)
+
+    def _torch_hyper(self, groups, steps):
+        """(lr, weight decay, AdamW step, lr_scales, weight decays) from a torch.optim state's param groups and the step
+        counts of its parameters.  Raises ValueError for what the fused optimizers cannot represent."""
+        for g in groups:
+            for key in ("nesterov", "amsgrad", "maximize"):
+                if g.get(key, False):
+                    raise ValueError(f"the torch.optim state sets {key}, which the fused optimizers do not offer")
+            if g.get("dampening", 0) != 0:
+                raise ValueError(f"the torch.optim state has dampening={g['dampening']}; the fused SGD has none")
+        keys = ("betas", "eps") if self.optimizer == "adamw" else ("momentum",)
+        for key in keys:
+            if any(tuple(g[key]) != tuple(groups[0][key]) if key == "betas" else g[key] != groups[0][key] for g in groups):
+                raise ValueError(f"the torch.optim state's param groups differ in {key}; the engine has one for all groups")
+        if len(steps) > 1:
+            raise ValueError(f"the torch.optim state's parameters are at different AdamW steps {sorted(steps)}; the "
+                             "engine keeps one step count")
+        lrs = [_check_group_value("lr", g["lr"]) for g in groups]
+        wds = [_check_group_value("weight_decay", g["weight_decay"]) for g in groups]
+        lr = lrs[-1]
+        if lr == 0 and any(v > 0 for v in lrs):
+            raise ValueError("the torch.optim state's last param group has lr 0 and another one not: the engine's lr is "
+                             "the last group's and every group's lr a multiple of it")
+        scales = [v / lr if lr else 1.0 for v in lrs]
+        return lr, wds[-1], int(steps.pop()) if steps else 0, scales, wds
+
+    def _restore_hyper(self, lr, weight_decay, group: dict, scales, wds, step: int) -> None:
+        """Set the hyper-parameters (momentum / betas, eps and LARS's trust coefficient from the param group `group`) and
+        refresh the device blocks, so that a captured CUDA graph follows."""
+        self.lr, self.weight_decay = lr, weight_decay
+        if self._groups is not None:
+            self._group_scale, self._group_wd = scales, wds
+        if self.optimizer == "adamw":
+            self.betas, self.eps = tuple(group["betas"]), group["eps"]
+            self._hp.copy_(torch.tensor(self._adamw_hp(step), dtype=torch.float32))
             self._write_groups()
             return
+        self.momentum = group["momentum"]
         if self.optimizer == "lars":
-            self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
-            self.trust_coefficient, self.eps = state["trust_coefficient"], state["eps"]
+            self.trust_coefficient, self.eps = group["trust_coefficient"], group["eps"]
             self._hp.copy_(torch.tensor(self._lars_hp(), dtype=torch.float32))
-            return
-        self.lr, self.momentum, self.weight_decay = state["lr"], state["momentum"], state["weight_decay"]
-        if self._hp is not None:
-            self.set_lr(self.lr)              # hyper-parameters live in device memory: refresh them
+        elif self._hp is not None:
+            self.set_lr(self.lr)              # hyper-parameters live in device memory: refresh them (and the group table)
         else:
             self._graph = None                # hyper-parameters are baked into a captured step
 

@@ -29,7 +29,9 @@ def main():
     ap.add_argument("--no-decay-1d", action="store_true",
                     help="no weight decay on biases and normalisation weights (torchvision's --norm-weight-decay 0.0)")
     ap.add_argument("--model", default="vgg16")
-    ap.add_argument("--checkpoint", default="")
+    ap.add_argument("--checkpoint", default="", help="save the model and the whole optimizer state here at the end")
+    ap.add_argument("--resume", default="",
+                    help="start from a --checkpoint file, saved at any number of GPUs (every rank loads it)")
     a = ap.parse_args()
     init_process_group_from_env()
     rank = int(os.environ.get("RANK", "0"))
@@ -39,6 +41,14 @@ def main():
                      param_groups=no_weight_decay_groups(model) if a.no_decay_1d else None)
     engine.enable_cuda_graph(True)            # forward + backward + every bucket kernel replay as one graph
     engine.set_lr(0.01)                       # hyper-parameters live in device memory: the graph follows the schedule
+    first = 0
+    if a.resume:
+        ck = torch.load(a.resume, map_location="cpu")
+        model.load_state_dict(ck["model"])
+        engine.load_full_optimizer_state_dict(ck["optimizer"])   # this rank's shards, whatever the saving world size
+        first = ck.get("step", 0)
+        if rank == 0:
+            print(f"resumed from {a.resume} at step {first}")
     last = []
 
     def remember(it):                         # (the last batch, for the evaluation on the EMA weights below)
@@ -46,7 +56,7 @@ def main():
             last[:] = [b]
             yield b
 
-    for step, loss in enumerate(engine.train_from_host(remember(batches(a.steps, a.batch, rank)))):
+    for step, loss in enumerate(engine.train_from_host(remember(batches(a.steps, a.batch, rank))), start=first):
         if step % 10 == 0:
             engine.set_lr(0.01 * 0.5 ** (step // 20))
             if rank == 0:
@@ -59,8 +69,10 @@ def main():
         model.train()
         if rank == 0:
             print(f"last batch on the EMA weights: loss {ema_loss:.4f}")
-    if a.checkpoint and rank == 0:
-        torch.save({"model": model.state_dict(), "optimizer": engine.optimizer_state_dict()}, a.checkpoint)
+    if a.checkpoint:
+        state = engine.full_optimizer_state_dict()            # collective: rank 0 gets the whole state, the others None
+        if rank == 0:
+            torch.save({"model": model.state_dict(), "optimizer": state, "step": first + a.steps}, a.checkpoint)
 
 
 if __name__ == "__main__":
